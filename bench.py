@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — SUPIR EDM sampling hot path on B200: megapixels/sec and ms/EDM-step.
+"""bench.py — SUPIR EDM sampling hot path on H100: megapixels/sec and ms/EDM-step.
 
 Default workload = BASELINE.json configs[2] ("cfg3", the configuration the metric is quoted on; it fits one GPU): one
 1024x1024 image restored at upscale 4 -> 4096x4096 output (16.78 MP), latent 512x512, `TiledRestoreEDMSampler(tile 128,
@@ -97,27 +97,19 @@ def workload_geometry(w):
 
 
 def peaks():
+    """bf16 dense tensor peak (TFLOP/s) and HBM bandwidth (GB/s) the roofline fractions are taken against: a measured
+    MEASURED_PEAKS.json next to this file if present, else the H100 SXM data sheet (700 W part; a card at a lower power
+    limit sustains less)."""
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             p = json.load(f)
         return p["bf16_tflops_sustained"], p["bf16_tflops"], p["hbm_gbs"], "measured"
     except Exception:
-        return 1400.0, 1590.0, 6650.0, "fallback"
-
-
-def load_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed ncu capture."""
-    for name in ("r02_gemm_traffic.json", "r01_gemm_traffic.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                return json.load(f)["dram_bytes_per_launch_mean"], name
-        except Exception:
-            continue
-    return None, None
+        return 989.0, 989.0, 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
 
     def __init__(self, index):
         self.index, self.proc, self.lines, self.i0 = index, None, [], 0
@@ -372,7 +364,9 @@ def engine_config(w, tile_batch):
 def build_engine(w, device, world):
     """supir_b200.model.SUPIRModel (the reference's SUPIRModel surface) with random bf16 weights of the real architecture."""
     from supir_b200 import model as smodel
-    tile_batch = int(os.environ.get("SUPIR_BENCH_TILE_BATCH", "49"))
+    # windows per network call: 17 runs cfg3's 49 windows as three calls (17 / 16 / 16 windows x CFG pair); one 98-row call
+    # per step does not leave room on an 80 GB H100 for its captured activations next to the VAE decoder's scratch
+    tile_batch = int(os.environ.get("SUPIR_BENCH_TILE_BATCH", "17"))
     with torch.device(device):
         m = smodel.SUPIRModel(**engine_config(w, tile_batch))
     m.model.diffusion_model.to(torch.bfloat16)
@@ -386,7 +380,7 @@ def build_engine(w, device, world):
 
 
 def profile_dominant_kernel(net, device):
-    """Live roofline of the dominant kernel (the tcgen05 GEMM / implicit-GEMM conv): one eager denoiser call with a
+    """Live roofline of the dominant kernel (the wgmma GEMM / implicit-GEMM conv): one eager denoiser call with a
     CUDA-event pair (current stream) around every GEMM-class launch of the plan the timed steps replayed; achieved = sum of
     the launches' algorithmic FLOPs / sum of their durations."""
     from supir_b200 import ops
@@ -527,6 +521,8 @@ def run_supir(args):
     if prof:
         torch.cuda.profiler.stop()
     step_ms = t0.elapsed_time(t1) / args.steps
+    # what the timed path computed in its last step: the sampler state x a caller of run.step() receives
+    dumped = {"latent": run.x.detach().float().cpu().numpy()} if args.dump_outputs else None
     lc1 = _native.launch_count() + net.replayed_launches
     clk = clocks.stop() if rank == 0 else None
     # ---- e2e steps: host latent in, host latent out, every step ----
@@ -597,14 +593,13 @@ def run_supir(args):
     # ---- roofline of the dominant kernel + CPU baseline (rank 0, N = 1 only) ----
     roof, cpu = None, None
     prof = profile_dominant_kernel(net, device)
-    traffic, traffic_src = load_traffic()
     ranks_on_step = world if shards else 1
     if prof is not None:
         g_flops, g_ms, g_n, g_key = prof
         achieved = g_flops / (g_ms * 1e-3) / 1e12
-        roof = {"bound": "tensor", "kernel": "supir::gemm_tcgen05_kernel (Linear / conv1x1 / implicit-GEMM conv3x3)",
-                "achieved": achieved, "peak": sust, "peak_kind": f"bf16 dense sustained, {peak_kind}", "unit": "TFLOP/s",
-                "frac": achieved / sust, "traffic": traffic, "traffic_unit": f"bytes/launch (mean of the ncu --set full capture profiles/{traffic_src})",
+        roof = {"bound": "tensor", "kernel": "supir::gemm_wgmma_kernel (Linear / conv1x1 / implicit-GEMM conv3x3)",
+                "achieved": achieved, "peak": sust, "peak_kind": f"bf16 dense, {peak_kind}", "unit": "TFLOP/s",
+                "frac": achieved / sust,
                 "launches_timed": g_n, "plan_batch_h_w_ctx": list(g_key),
                 "step_flops": step_flop, "step_achieved_tflops": step_flop / (step_ms * 1e-3) / 1e12,
                 "step_frac_of_peak": step_flop / (step_ms * 1e-3) / 1e12 / (sust * ranks_on_step)}
@@ -628,7 +623,7 @@ def run_supir(args):
         "config": {"workload": f"{args.config}: " + w["desc"] + "; SUPIR-v0 + SDXL-base + SDXL-VAE shapes, random weights",
                    "sampler_steps": w["steps"], "windows": windows, "tile_batch": getattr(smp, "tile_batch", None), "images": images,
                    "vae_ms": vae_ms, "vae_pre_ms": vae_pre_ms, "vae_post_ms": vae_post_ms, "vae_warmup_passes": min(args.warmup, 1), "vae_warmup": "one untimed denoise-encode + decode + encode (fills the three networks' scratch pools)",
-                   "l2": "per-step working set (7.7 GB of weights + activations) exceeds the 126 MB L2",
+                   "l2": "per-step working set (7.7 GB of weights + activations) exceeds the 50 MB L2",
                    "output_finite": finite, "vae_skipped_INVALID_FOR_BENCH": skip_vae,
                    "parallelism": (f"(CFG branch, window) units and VAE tiles sharded over {world} rank(s), 1 all-gather/step" if shards else
                                    (f"{world} independent replicas" if world > 1 else "single GPU"))},
@@ -643,6 +638,11 @@ def run_supir(args):
     }
     if cpu is not None:
         line["cpu_baseline"] = cpu
+    if dumped is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dumped.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
+        line["dumped_outputs"] = {name: list(arr.shape) for name, arr in dumped.items()}
     print(json.dumps(line))
     if world > 1:
         dist.barrier()
@@ -658,6 +658,8 @@ def main():
     ap.add_argument("--config", default="cfg3", choices=sorted(WORKLOADS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-full-run", action="store_true", help="skip the one real batchify_sample run of the whole configuration")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the sampler latent of the last timed step (float32) as DIR/latent.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "supir_b200" else args.warmup
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-/* supir_b200 — C ABI of the B200 (sm_100a) backend for SUPIR's EDM sampling hot path.
+/* supir_b200 — C ABI of the H100 (sm_90a) backend for SUPIR's EDM sampling hot path.
  *
  * The reference (Fanghua-Yu/SUPIR) has no FFI: its hot path is a tree of torch.nn modules that dispatch to
  * cuDNN/cuBLAS/ATen. This header is the boundary a maintainer binds instead (ctypes stub in INTEGRATION.md): each entry
@@ -29,7 +29,7 @@ long long supir_launch_count(void);
 void supir_reset_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------------------------ */
-/* K2/K3/K4: Linear, conv1x1, conv3x3 on tcgen05 tensor cores (gemm.cu)                                               */
+/* K2/K3/K4: Linear, conv1x1, conv3x3 on wgmma tensor cores (gemm.cu)                                                 */
 /* ------------------------------------------------------------------------------------------------------------------ */
 typedef struct supir_epilogue {
     const float* bias;      /* [N] fp32 or NULL                      (nn.Linear / nn.Conv2d bias)                      */
@@ -83,20 +83,6 @@ int supir_conv_geom_bf16(const void* x, long long ldx, const void* Wp, void* out
 
 /* debugging / tuning knob: force the N tile (64/128/256), 0 = heuristic */
 int supir_set_gemm_tile_n(int bn);
-/* tuning knob: the widest tile can run on CTA pairs (2-CTA clusters, tcgen05 cta_group::2: a 256 x 256 tile per pair,
- * each CTA staging half of the W tile). 0 = single-CTA kernel everywhere, 1 = pairs where they measured faster (default;
- * also settable through the environment variable SUPIR_B200_GEMM_PAIR), 2 = pairs whenever the tile is 256 wide */
-int supir_set_gemm_pair_mode(int on);
-/* tuning knob for the staged epilogue: 0 = one TMA load / store per 128-row chunk, issued by one thread of each 4-warp group
- * behind two named barriers; 1 = every epilogue warp moves its own 32 rows with its own TMA operations and mbarriers, no
- * cross-warp barrier in the chunk loop; negative = environment (SUPIR_B200_GEMM_WARP_EPILOGUE) or, by default, automatic:
- * per-warp for every epilogue except GEGLU (measured: profiles/r02_selftest_epiperf.log). */
-int supir_set_gemm_epilogue_mode(int per_warp);
-/* debugging: 1 routes every GEMM through the direct-store epilogue instead of the shared-memory + TMA-store one */
-int supir_debug_force_direct_epilogue(int on);
-/* debugging: override the UMMA shared-memory descriptor template / instruction descriptor (-1 = built-in default) */
-int supir_debug_set_umma_descriptors(long long smem_desc_template, long long idesc);
-
 /* ------------------------------------------------------------------------------------------------------------------ */
 /* network entry / exit convolutions with < 8 channels on one side (smallconv.cu)                                     */
 /* ------------------------------------------------------------------------------------------------------------------ */
@@ -171,7 +157,6 @@ int supir_softmax_rows(const float* S, long long lds, void* P, long long ldp, lo
  * ZeroCrossAttn (SUPIR_v0.py:146). */
 int supir_attention_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                          void* out, long long ldo, int B, int H, int Lq, int Lk, int head_dim, float scale, void* stream);
-int supir_debug_set_attention_descriptors(long long smem_desc_template, long long idesc_pv);
 /* Single-head attention with a wide head over L tokens per batch element (the SDXL VAE mid-block AttnBlock, head_dim 512:
  * model.py:158-206, 209-262; tilevae.py:292-336; 128 / 256 for reduced-width VAE configurations):
  * out[b, i, 0:head_dim] = softmax(q k^T * scale) v. q/k/v/out: [B*L, ld] bf16, ld >= head_dim. Flash-style (no score matrix
@@ -179,13 +164,8 @@ int supir_debug_set_attention_descriptors(long long smem_desc_template, long lon
 int supir_attention_1head_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                                void* out, long long ldo, int B, int L, int head_dim, float scale, void* stream);
 /* tuning knob: how many of every 4 element pairs of the softmax take 2^x from the FMA-pipe polynomial instead of MUFU.EX2
- * (0..4; default 0 = all on MUFU, which measured fastest on B200, or the environment variable SUPIR_B200_ATTN_EMU; negative
- * restores the default). */
+ * (0..4; default 0 = all on MUFU, or the environment variable SUPIR_B200_ATTN_EMU; negative restores the default). */
 int supir_set_attention_exp_emulation(int pairs_of_4);
-/* tuning knob: cycles by which the second query tile of a self-attention CTA starts behind the first, so that the two tiles'
- * softmax phases interleave on the shared MUFU instead of running in lockstep (environment SUPIR_B200_ATTN_STAGGER; negative
- * restores the default). */
-int supir_set_attention_stagger(int cycles);
 /* tuning knob: how many of every 4 probability pairs are rounded / packed to bf16 with integer instructions on the ALU pipe
  * instead of cvt.rn.bf16x2.f32, which shares the XU pipe with the exponentials (0..4; environment SUPIR_B200_ATTN_ALU_PACK;
  * negative restores the default). */

@@ -1,4 +1,4 @@
-"""supir_b200 — B200 (sm_100a) backend for SUPIR's EDM sampling hot path.
+"""supir_b200 — H100 (sm_90a) backend for SUPIR's EDM sampling hot path.
 
 Hand-written CUDA kernels behind a C ABI (include/supir_b200.h, supir_b200/csrc/), driven by host classes that mirror
 the reference's sgm / SUPIR plugin surface (same class names, constructor parameters, state_dict keys and call

@@ -30,10 +30,6 @@ _SIGS = {
     "supir_conv_geom_bf16": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(ConvGeometry),
                              ctypes.POINTER(Epilogue), c_void_p],
     "supir_set_gemm_tile_n": [c_int],
-    "supir_set_gemm_pair_mode": [c_int],
-    "supir_set_gemm_epilogue_mode": [c_int],
-    "supir_debug_force_direct_epilogue": [c_int],
-    "supir_debug_set_umma_descriptors": [c_ll, c_ll],
     "supir_conv3x3_small_cin": [c_void_p, c_ll, c_ll, c_ll, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "supir_im2col_3x3_small_cin": [c_void_p, c_ll, c_ll, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "supir_conv3x3_small_cout": [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
@@ -48,9 +44,7 @@ _SIGS = {
     "supir_softmax_rows": [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_int, c_float, c_void_p],
     "supir_attention_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p],
     "supir_attention_1head_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_float, c_void_p],
-    "supir_debug_set_attention_descriptors": [c_ll, c_ll],
     "supir_set_attention_exp_emulation": [c_int],
-    "supir_set_attention_stagger": [c_int],
     "supir_set_attention_alu_pack": [c_int],
     "supir_upsample_nearest2x": [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p],
     "supir_im2col_3x3_s2": [c_void_p, c_ll, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],

@@ -3,7 +3,7 @@
 The reference resolves every hot-path class by dotted string through `sgm.util.instantiate_from_config`
 (sgm/util.py:168-185) and `get_obj_from_str` (sgm/models/diffusion.py:50-53). `install()` imports the reference's own
 modules and rebinds those names to this package's classes, so `test.py` / `gradio_demo_tiled.py` — which only touch the
-object returned by `create_SUPIR_model` — run unchanged on the B200 backend:
+object returned by `create_SUPIR_model` — run unchanged on the H100 backend:
 
     python -c "import supir_b200.compat as c; c.install(); import runpy; runpy.run_path('test.py', run_name='__main__')" ...
 

@@ -1,4 +1,4 @@
-"""Text conditioner on the B200 backend (SURVEY.md §8(f)2): `GeneralConditioner` / `GeneralConditionerWithControl`,
+"""Text conditioner on the H100 backend (SURVEY.md §8(f)2): `GeneralConditioner` / `GeneralConditionerWithControl`,
 `FrozenCLIPEmbedder` (CLIP ViT-L/14 text tower), `FrozenOpenCLIPEmbedder2` (OpenCLIP ViT-bigG/14 text tower) and
 `ConcatTimestepEmbedderND` with the reference's class names, constructor parameters, state_dict keys and outputs
 (sgm/modules/encoders/modules.py:81-243, 445-609, 1027-1043; wired by options/SUPIR_v0.yaml:66-105).
@@ -7,7 +7,7 @@ The reference runs the two towers through third-party packages (transformers==4.
 `open_clip.create_model_and_transforms`) under fp16 autocast, once per image for the positive and once for the negative prompt.
 Here the torch modules only OWN the parameters (HF / open_clip key layout, so SUPIR checkpoints and the upstream CLIP weight
 files load unchanged) and `forward()` drives this library's kernels: fp32 residual stream like the reference (autocast
-lowers only the matmuls), LayerNorm -> bf16, fused QKV projection on the tcgen05 GEMM, causal attention, out-projection / MLP
+lowers only the matmuls), LayerNorm -> bf16, fused QKV projection on the wgmma GEMM, causal attention, out-projection / MLP
 GEMMs with fp32 output accumulated into the stream. There is no torch compute fallback.
 
 Tokenisation (host-side string processing) is native too — supir_b200/clip_bpe.py, CLIP's byte-level BPE with the two layouts the

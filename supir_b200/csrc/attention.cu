@@ -1,35 +1,28 @@
-// supir_b200 — K6 of SURVEY.md §2a: softmax(Q K^T / sqrt(d)) V for head_dim 64, no mask, on tcgen05.
+// supir_b200 — K6 of SURVEY.md §2a: softmax(Q K^T / sqrt(d)) V without mask, flash-style on Hopper wgmma.
 //
 // Replaces F.scaled_dot_product_attention / xformers.memory_efficient_attention in CrossAttention
 // (sgm/modules/attention.py:273-277, 357-359) for self-attention, 77-token cross-attention and ZeroCrossAttn
-// (SUPIR/modules/SUPIR_v0.py:146).
+// (SUPIR/modules/SUPIR_v0.py:146), and the single-head attention of the SDXL VAE's mid block
+// (sgm/modules/diffusionmodules/model.py:158-206 / MemoryEfficientAttnBlock :209-262; per tile in SUPIR/utils/tilevae.py:292-336).
 //
-// PERSISTENT kernel: one CTA per SM (two for the one-tile variant) walks work items (batch, head, query block) with stride
-// gridDim.x; barriers and TMEM are set up once. 128 + 128*TILES threads, warp-specialised:
-//   warp 0 lane 0 : TMA producer. Q of the NEXT item is fetched into the second Q buffer while the current item computes;
-//                   K/V 128-row blocks run through one ring that simply continues across items.
-//   warp 1 lane 0 : tcgen05.mma issuer. Per tile X (128 query rows) and key block j:
-//                     S_X = Q_X K_j^T   (128 x NKEY x 64, TMEM, overwritten every block)
-//                     O_X += P_X V_j    (128 x 64 x NKEY, ACCUMULATED in TMEM across the blocks of an item)
-//                   with P_X read straight from TENSOR MEMORY (A-in-TMEM form of tcgen05.mma: P never touches shared
-//                   memory, whose bandwidth the QK/PV operand reads already saturate) and V consumed in its natural
-//                   [kv, d] layout as an MN-major B operand. The first QK of the next item is issued while the softmax
-//                   warps still normalise and store the current item's O.
-//   warps 4..7    : softmax group of tile A, warps 8..11: tile B — one query row per thread. The whole S row is read from
-//                   TMEM once into registers; p = 2^((s - m) * scale) is packed to bf16 pairs and stored back to TMEM
-//                   (tcgen05.st) as the A operand of the PV MMA.
-// The softmax is the bound of this kernel, not the MMA: at head_dim 64 a key block costs 512 tensor-pipe cycles per tile but
-// 128 ex2 per row = 1024 MUFU cycles per warp (MUFU: 4 lanes/clk per SM sub-partition). So
-//   * the arithmetic around the exponential runs on PACKED fp32 pairs (fma/add.f32x2 -> FFMA2/FADD2: half the issue slots);
-//   * (optional, OFF by default — it measured slower on B200, see attention_emu()) EMU of every 4 element pairs can take
-//     their exponential on the FMA pipe instead of MUFU: Cody-Waite split
-//     x = n + f (add.rm with the 1.5*2^23 magic constant), degree-3 minimax polynomial for 2^f on [0,1) (max rel. error
-//     8.8e-5 = 2^-13.5, far below the bf16 rounding of P at 2^-9), exponent reinserted with one integer shift-add;
-//   * the row maximum uses 3-input FMNMX3; online softmax never touches O in the common case: the exponent reference m is
-//     only moved when the running row maximum exceeds it by more than 8 (p <= 2^8 stays exact enough in bf16/fp32); only
-//     then the warp rescales its 32 rows of O in TMEM and its row sum.
+// One kernel template serves both: a CTA owns 128 queries of one (batch, head) and DV = 64 * NVC value columns of it;
+// 384 threads = three warpgroups:
+//   warpgroup 0, thread 0 : TMA producer. Q (128 x D, as D / 64 chunks of 64 columns, 128B-swizzled) once; then K and V
+//                           blocks of BKV keys through one ring of slots, in the order the consumers use them:
+//                           K(j) chunks 0..NCH-1, V(j) chunks 0..NVC-1, K(j+1) ...
+//   warpgroups 1, 2       : 64 query rows each. Per key block j:
+//                             S = Q K_j^T       wgmma m64 x BKV, A and B from shared memory (both K-major)
+//                             online softmax on the S fragment in registers (row max / sum across the 4 threads of a row)
+//                             O += P V_j        wgmma m64 x 64 per value chunk, A = P straight from registers (the S
+//                                               fragment repacked to bf16: accumulator and A-operand layouts coincide),
+//                                               B = V in its natural [key, channel] layout (MN-major, transposed operand)
+//                           and finally O / l stored as bf16.
+// Head dim 64 (multi-head): NCH = NVC = 1, BKV = 128. The VAE's single head of 512 channels: Q stays resident (128 KB),
+// BKV = 64 keys per block (S: 32 registers per thread next to 128 of O), the 512 value columns split over two CTAs
+// (grid.y), which both compute Q K^T.
 #include "common.cuh"
 #include "supir_b200.h"
+#include "wgmma.cuh"
 
 #include <cstdlib>
 
@@ -38,410 +31,243 @@ namespace supir {
 int make_tmap_bf16(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
                    const uint32_t* box);
 
-static constexpr int ATT_BM = 128;   // queries per tile
-static constexpr int ATT_BN = 128;   // keys per block
-static constexpr int ATT_D = 64;
-static constexpr float ATT_RESCALE_THRESHOLD = 8.0f;   // log2 units
+static constexpr int ATT_BM = 128;   // queries per CTA (64 per consumer warpgroup)
+static constexpr int ATT_THREADS = 384;
 
 struct AttnParams {
-    int Lq, Lk, H;
+    int Lq, Lk;
+    int nsplit;            // CTAs sharing one head's value columns (grid.y = heads * nsplit)
+    int head_cols;         // columns of one head in q / k / v / out
     long long ldo;
     __nv_bfloat16* out;
     float scale_log2;
-    uint32_t desc_hi;      // smem descriptor template (upper word)
-    uint32_t idesc_qk;     // 128 x NKEY, A K-major, B K-major
-    uint32_t idesc_pv;     // 128 x 64,  A K-major (TMEM), B MN-major
-    int nqb, num_items;    // query blocks per (batch, head); nqb * H * B work items
-    int stagger;           // cycles by which tile B's first QK trails tile A's (see attention_stagger())
 };
 
-// 2^x for a pair, x <= ~100, on the FMA / ALU pipes (no MUFU). x is clamped at -126 (result 2^-126 ~ 0 for anything below,
-// including the -inf of masked keys).
-__device__ __forceinline__ void ex2_emulated_pair(uint64_t x, float& e0, float& e1) {
+// 2^x on the FMA / ALU pipes (no MUFU). x is clamped at -126 (result 2^-126 ~ 0 for anything below, including the -inf
+// of masked keys): Cody-Waite split x = n + f (round-down add of the 1.5*2^23 magic constant), degree-3 minimax
+// polynomial for 2^f on [0,1) (max rel. error 8.8e-5 = 2^-13.5, far below the bf16 rounding of P at 2^-9), exponent
+// reinserted with one integer shift-add.
+__device__ __forceinline__ float ex2_emulated(float x) {
     const float kMagic = 12582912.0f;                       // 1.5 * 2^23: x + magic has ulp 1, floor(x) lands in the low mantissa bits
-    float x0, x1;
-    unpack2(x, x0, x1);
-    x0 = fmaxf(x0, -126.0f);
-    x1 = fmaxf(x1, -126.0f);
-    const uint64_t xc = pack2(x0, x1);
-    const uint64_t xr = fadd2_rm(xc, pack2(kMagic, kMagic));            // magic + floor(x)
-    const uint64_t xf = fadd2(xr, pack2(-kMagic, -kMagic));             // floor(x), exact
-    const uint64_t fr = ffma2(xf, pack2(-1.0f, -1.0f), xc);             // x - floor(x) in [0, 1), exact
-    uint64_t p = ffma2(pack2(0.077119089663028717041015625f, 0.077119089663028717041015625f), fr,
-                       pack2(0.227564394474029541015625f, 0.227564394474029541015625f));
-    p = ffma2(p, fr, pack2(0.695146143436431884765625f, 0.695146143436431884765625f));
-    p = ffma2(p, fr, pack2(1.0f, 1.0f));                                // 2^f in [1, 2]
-    float p0, p1, r0, r1;
-    unpack2(p, p0, p1);
-    unpack2(xr, r0, r1);
+    x = fmaxf(x, -126.0f);
+    const float xr = __fadd_rd(x, kMagic);                  // magic + floor(x)
+    const float xf = __fadd_rn(xr, -kMagic);                // floor(x), exact
+    const float fr = __fadd_rn(x, -xf);                     // x - floor(x) in [0, 1), exact
+    float p = fmaf(0.077119089663028717041015625f, fr, 0.227564394474029541015625f);
+    p = fmaf(p, fr, 0.695146143436431884765625f);
+    p = fmaf(p, fr, 1.0f);                                  // 2^f in [1, 2]
     // bits(magic + n) = 0x4B400000 + n: the low 9 bits of the constant are zero, so << 23 leaves n in the exponent field
-    e0 = __uint_as_float(__float_as_uint(p0) + (__float_as_uint(r0) << 23));
-    e1 = __uint_as_float(__float_as_uint(p1) + (__float_as_uint(r1) << 23));
+    return __uint_as_float(__float_as_uint(p) + (__float_as_uint(xr) << 23));
 }
 
 // fp32 pair -> bf16x2 with INTEGER arithmetic: round half up on the magnitude (+0x8000, p >= 0) and take the two high halves
-// with one byte permute. cvt.rn.bf16x2.f32 (F2FP) runs on the same XU pipe as the exponentials — 64 pack instructions
-// per row and block are a fifth of this kernel's XU time — while the ALU pipe these three instructions use is mostly idle.
-// Differs from round-to-nearest-even only on exact ties.
+// with one byte permute, on the ALU pipe instead of the conversion unit. Differs from round-to-nearest-even only on exact ties.
 __device__ __forceinline__ uint32_t pack_bf16x2_alu(float lo, float hi) {
     return __byte_perm(__float_as_uint(lo) + 0x8000u, __float_as_uint(hi) + 0x8000u, 0x7632);
 }
 
-// p = 2^(s * scale - m) for NCOL columns of one row (registers s[]), bf16 pairs to TMEM at tP; returns the row sum of p.
-// EMU of every 4 pairs are evaluated by ex2_emulated_pair, the others on MUFU; ICVT of every 4 pairs are packed to bf16 on
-// the ALU pipe (pack_bf16x2_alu), the others by the XU-pipe conversion instruction.
-template <int NCOL, int EMU, int ICVT>
-__device__ __forceinline__ float softmax_row_to_tmem(const uint32_t (&s)[128], float scale_log2, float m_ref, uint32_t tP) {
-    const uint64_t sc2 = pack2(scale_log2, scale_log2), nm2 = pack2(-m_ref, -m_ref);
-    uint64_t ls[4];
-#pragma unroll
-    for (int t = 0; t < 4; ++t) ls[t] = 0ull;
-#pragma unroll
-    for (int c0 = 0; c0 < NCOL; c0 += 64) {
-        uint32_t pk[32];                                     // 64 probabilities as bf16 pairs
-#pragma unroll
-        for (int i = 0; i < 64; i += 8) {
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-                const int c = c0 + i + 2 * t;
-                if (c < NCOL) {
-                    const uint64_t x = ffma2(pack2(__uint_as_float(s[c]), __uint_as_float(s[c + 1])), sc2, nm2);
-                    float e0, e1;
-                    // spread the emulated pairs over the group so MUFU and FMA work interleave in the instruction stream
-                    const bool emulate = (EMU == 4) || (EMU == 3 && t != 1) || (EMU == 2 && (t & 1)) || (EMU == 1 && t == 3);
-                    if (emulate) {
-                        ex2_emulated_pair(x, e0, e1);
-                    } else {
-                        float x0, x1;
-                        unpack2(x, x0, x1);
-                        e0 = ex2_approx(x0);
-                        e1 = ex2_approx(x1);
-                    }
-                    ls[t] = fadd2(ls[t], pack2(e0, e1));
-                    const bool alu_pack = (ICVT == 4) || (ICVT == 2 && !(t & 1)) || (ICVT == 1 && t == 0) || (ICVT == 3 && t != 2);
-                    pk[(i >> 1) + t] = alu_pack ? pack_bf16x2_alu(e0, e1) : pack_bf16x2(e0, e1);
-                } else {
-                    pk[(i >> 1) + t] = 0u;
-                }
-            }
-        }
-        tmem_st_32x32(tP + (c0 >> 1), pk);
-    }
-    tmem_st_wait();
-    float a0, a1;
-    unpack2(fadd2(fadd2(ls[0], ls[1]), fadd2(ls[2], ls[3])), a0, a1);
-    return a0 + a1;
-}
-
-// TILES = 128-query tiles per CTA, STAGES = K/V ring depth, NKEY = key columns computed per block (128; 96 when every key
-// fits in 96 rows, i.e. the 77-token text cross-attention), EMU = emulated pairs per 4 (see above).
-template <int TILES, int STAGES>
+template <int NCH, int NVC, int BKV>
 struct AttnSmem {
-    static constexpr int Q_BYTES = ATT_BM * ATT_D * 2;          // 16 KB per tile
-    static constexpr int K_BYTES = ATT_BN * ATT_D * 2;          // 16 KB
-    static constexpr int V_BYTES = ATT_BN * ATT_D * 2;          // 16 KB
-    static constexpr int OFF_Q = 0;                              // [2 items][TILES]
-    static constexpr int OFF_K = OFF_Q + 2 * TILES * Q_BYTES;
-    static constexpr int OFF_V = OFF_K + STAGES * K_BYTES;
-    static constexpr int OFF_BAR = OFF_V + STAGES * V_BYTES;
+    static constexpr int Q_CHUNK = ATT_BM * 64 * 2;                 // 16 KB: 128 rows x 64 bf16
+    static constexpr int SLOT = BKV * 64 * 2;                        // one K or V chunk: BKV rows x 64 bf16
+    static constexpr int SLOTS = (NCH > NVC ? NCH : NVC) + 2 > 6 ? (NCH > NVC ? NCH : NVC) + 2 : 6;
+    static constexpr int OFF_RING = NCH * Q_CHUNK;
+    static constexpr int OFF_BAR = OFF_RING + SLOTS * SLOT;
     static constexpr int TOTAL = OFF_BAR + 256 + 1024;
 };
 
-template <int TILES, int STAGES, int NKEY, int EMU, int ICVT>
-__global__ void __launch_bounds__(128 + 128 * TILES, TILES == 1 ? 2 : 1)
-attention_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
-    using SM = AttnSmem<TILES, STAGES>;
-    constexpr uint32_t TMEM_COLS = TILES == 2 ? 512 : 256;
-    // TMEM columns: S_A [0,128) S_B [128,256) O_A [256,320) O_B [320,384) P_A [384,448) P_B [448,512) (bf16 pairs)
-    constexpr uint32_t COL_O = TILES * ATT_BN, COL_P = TILES * ATT_BN + TILES * ATT_D;
-    constexpr uint32_t KV_TX = (uint32_t)NKEY * ATT_D * 2 * 2;          // bytes of one K + V block as the tensor-map box delivers it
+template <int BKV>
+__device__ __forceinline__ void wgmma_qk(float (&s)[BKV / 2], uint64_t da, uint64_t db, int scale_d) {
+    if constexpr (BKV == 128) wgmma_ss_n128(s, da, db, scale_d);
+    else wgmma_ss_n64(s, da, db, scale_d);
+}
+
+// NCH = 64-column chunks of the head dim (Q K^T depth), NVC = 64-column value chunks per CTA, BKV = keys per block,
+// EMU = exponential pairs of every 4 evaluated by ex2_emulated, ICVT = probability pairs of every 4 packed on the ALU pipe
+template <int NCH, int NVC, int BKV, int EMU, int ICVT>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                       const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
+    using SM = AttnSmem<NCH, NVC, BKV>;
+    constexpr int SLOTS = SM::SLOTS;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sQ = smem + SM::OFF_Q;
-    uint8_t* sK = smem + SM::OFF_K;
-    uint8_t* sV = smem + SM::OFF_V;
+    uint8_t* sQ = smem;
+    uint8_t* ring = smem + SM::OFF_RING;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::OFF_BAR);
-    uint64_t* q_full = bars;                            // [2] per Q buffer
-    uint64_t* q_empty = bars + 2;                       // [2]
-    uint64_t* kv_full = bars + 4;                       // [STAGES]
-    uint64_t* kv_empty = kv_full + STAGES;              // [STAGES]
-    uint64_t* s_full = kv_empty + STAGES;               // [2] per tile
-    uint64_t* p_full = s_full + 2;                      // [2] per tile
-    uint64_t* pv_done = p_full + 2;                     // [2] per tile
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(pv_done + 2);
+    uint64_t* q_full = bars;                        // 1
+    uint64_t* slot_full = bars + 1;                 // [SLOTS]
+    uint64_t* slot_empty = slot_full + SLOTS;       // [SLOTS]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int nblk = (p.Lk + ATT_BN - 1) / ATT_BN;
-    // work item -> (batch, head, first query row); the same arithmetic in every role. Query blocks of one (batch, head) are
-    // consecutive items, so the CTAs running at the same time share that head's K/V in L2.
-    auto item_q0 = [&](int it) { return (it % p.nqb) * TILES * ATT_BM; };
-    auto item_head = [&](int it) { return (it / p.nqb) % p.H; };
-    auto item_batch = [&](int it) { return it / (p.nqb * p.H); };
-    auto item_tileB = [&](int it) { return TILES == 2 && (item_q0(it) + ATT_BM) < p.Lq; };
+    const int q0 = blockIdx.x * ATT_BM, head = blockIdx.y / p.nsplit, split = blockIdx.y % p.nsplit, batch = blockIdx.z;
+    const int nblk = (p.Lk + BKV - 1) / BKV;
+    const int qk_col = head * p.head_cols;                       // first Q / K column of this head
+    const int v_col = head * p.head_cols + split * NVC * 64;    // first value (and output) column of this CTA
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmQ);
         tma_prefetch_desc(&tmK);
         tma_prefetch_desc(&tmV);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&q_full[i], 1);
-            mbar_init(&q_empty[i], 1);
-            mbar_init(&s_full[i], 1);
-            mbar_init(&p_full[i], 4);
-            mbar_init(&pv_done[i], 1);
-        }
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
+        mbar_init(q_full, 1);
+        for (int s = 0; s < SLOTS; ++s) { mbar_init(&slot_full[s], 1); mbar_init(&slot_empty[s], 8); }   // 8 consumer warps
         fence_barrier_init();
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_ptr, TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
     if (warp < 4) {
-      // register budgets (the CTA's pool is what the launch reserved: 168 regs x 384 threads, or 128 x 256 with two CTAs per
-      // SM): <2,*> 64 control / 216 softmax, <1,*> 56 / 200. What the four control warps give up must cover what the softmax
-      // warps ask for, or the last setmaxnreg.inc waits forever: (168-64)*4 = 416 >= (216-168)*8 = 384; (128-56)*4 = (200-128)*4.
-      if (TILES == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
-      else asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-      if (warp == 0) {
-        if (lane == 0) {
-            // ---------------- TMA producer: runs ahead of the math by up to one item of Q and STAGES blocks of K/V ----------------
-            int stage = 0;
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (threadIdx.x == 0) {
+            mbar_expect_tx(q_full, NCH * SM::Q_CHUNK);
+            for (int c = 0; c < NCH; ++c) tma_load_2d(sQ + c * SM::Q_CHUNK, &tmQ, q_full, qk_col + c * 64, batch * p.Lq + q0);
+            int slot = 0;
             uint32_t phase = 0;
-            int k = 0;                                                   // local item counter
-            for (int it = blockIdx.x; it < p.num_items; it += gridDim.x, ++k) {
-                const int qi = k & 1;
-                const int head = item_head(it), batch = item_batch(it), q0 = item_q0(it);
-                const bool tb = item_tileB(it);
-                uint8_t* q_buf = sQ + qi * TILES * SM::Q_BYTES;
-                mbar_wait(&q_empty[qi], ((k >> 1) & 1) ^ 1);             // the item that used this buffer two items ago is done with it
-                mbar_expect_tx(&q_full[qi], (tb ? 2 : 1) * SM::Q_BYTES);
-                tma_load_2d(q_buf, &tmQ, &q_full[qi], head * ATT_D, batch * p.Lq + q0);
-                if (tb) tma_load_2d(q_buf + SM::Q_BYTES, &tmQ, &q_full[qi], head * ATT_D, batch * p.Lq + q0 + ATT_BM);
-                for (int j = 0; j < nblk; ++j) {
-                    mbar_wait(&kv_empty[stage], phase ^ 1);
-                    mbar_expect_tx(&kv_full[stage], KV_TX);
-                    tma_load_2d(sK + stage * SM::K_BYTES, &tmK, &kv_full[stage], head * ATT_D, batch * p.Lk + j * ATT_BN);
-                    tma_load_2d(sV + stage * SM::V_BYTES, &tmV, &kv_full[stage], head * ATT_D, batch * p.Lk + j * ATT_BN);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ---------------- MMA issuer ----------------
-            const uint64_t dtemplate = (uint64_t)p.desc_hi << 32;
-            auto issue_qk = [&](int x, int qi, int stage) {
-                const uint64_t qdesc = dtemplate | ((smem_u32(sQ + (qi * TILES + x) * SM::Q_BYTES) >> 4) & 0x3FFF);
-                const uint64_t kdesc = dtemplate | ((smem_u32(sK + stage * SM::K_BYTES) >> 4) & 0x3FFF);
-#pragma unroll
-                for (int kk = 0; kk < ATT_D / 16; ++kk)
-                    umma_bf16(tmem_base + x * ATT_BN, qdesc + 2 * kk, kdesc + 2 * kk, p.idesc_qk, kk != 0);
-                umma_commit(&s_full[x]);
+            auto push = [&](const CUtensorMap* tm, int col, int row) {
+                mbar_wait(&slot_empty[slot], phase ^ 1);
+                mbar_expect_tx(&slot_full[slot], SM::SLOT);
+                tma_load_2d(ring + slot * SM::SLOT, tm, &slot_full[slot], col, row);
+                if (++slot == SLOTS) { slot = 0; phase ^= 1; }
             };
-            int stage = 0;                 // stage holding the current block
-            uint32_t kv_phase = 0;
-            uint32_t g[2] = {0, 0};        // blocks processed per tile (parity of p_full)
-            int k = 0;
-            if ((int)blockIdx.x < p.num_items) {    // prologue: first QK of the first item
-                mbar_wait(&q_full[0], 0);
-                mbar_wait(&kv_full[0], 0);
-                tc_fence_after();
-                const int nt0 = item_tileB(blockIdx.x) ? 2 : 1;
-                issue_qk(0, 0, 0);
-                if (nt0 == 2) {
-                    // Start tile B out of phase with tile A. The two tiles' softmax warps share each sub-partition's MUFU: started
-                    // together they stay in lockstep — both in the exponential phase (each at half rate), then both waiting for
-                    // their next S while the MUFU idles. Offset by part of a softmax period, one tile's wait / load / max phase
-                    // hides behind the other's exponentials, and the offset persists (each tile's blocks chain independently).
-                    if (p.stagger > 0) {
-                        const long long t0 = clock64();
-                        while (clock64() - t0 < p.stagger) {}
-                    }
-                    issue_qk(1, 0, 0);
-                }
-            }
-            for (int it = blockIdx.x; it < p.num_items; it += gridDim.x, ++k) {
-                const int qi = k & 1;
-                const int ntile = item_tileB(it) ? 2 : 1;
-                const int it_next = it + gridDim.x;
-                const bool more_items = it_next < p.num_items;
-                const int ntile_next = more_items && item_tileB(it_next) ? 2 : 1;
-                for (int j = 0; j < nblk; ++j) {
-                    int nstage = stage + 1;
-                    uint32_t nphase = kv_phase;
-                    if (nstage == STAGES) { nstage = 0; nphase ^= 1; }
-                    const bool last = (j + 1 == nblk);
-                    const bool has_next = !last || more_items;       // a QK to issue ahead: next block, or the next item's first
-                    const int nqi = last ? (qi ^ 1) : qi;
-                    const int nt_next = last ? ntile_next : ntile;   // tiles of the item that owns the next block
-                    if (has_next) {
-                        if (last) mbar_wait(&q_full[nqi], ((k + 1) >> 1) & 1);
-                        mbar_wait(&kv_full[nstage], nphase);
-                    }
-                    for (int x = 0; x < TILES; ++x) {
-                        const bool cur = x < ntile, nxt = has_next && x < nt_next;
-                        if (cur) {
-                            mbar_wait(&p_full[x], g[x] & 1);     // P_X of this block written, S_X consumed
-                            tc_fence_after();
-                        }
-                        // tile B may sit out an item (ragged last query block): its S is then free already
-                        if (nxt) {
-                            if (!cur) tc_fence_after();
-                            issue_qk(x, nqi, nstage);
-                        }
-                        if (cur) {
-                            const uint32_t vbase = smem_u32(sV + stage * SM::V_BYTES);
-#pragma unroll
-                            for (int kk = 0; kk < NKEY / 16; ++kk) {
-                                // A = P in TMEM: 16 k-elements = 8 columns per step; B = V: MN-major (d contiguous), 16 kv rows of 128 B
-                                const uint32_t va = vbase + kk * 16 * 128;
-                                umma_bf16_ts(tmem_base + COL_O + x * ATT_D, tmem_base + COL_P + x * 64 + kk * 8,
-                                             dtemplate | ((va >> 4) & 0x3FFF), p.idesc_pv, (j | kk) != 0);
-                            }
-                            umma_commit(&pv_done[x]);
-                            ++g[x];
-                        }
-                    }
-                    umma_commit(&kv_empty[stage]);
-                    if (last) umma_commit(&q_empty[qi]);            // every QK of this item was issued before this point
-                    stage = nstage;
-                    kv_phase = nphase;
-                }
+            for (int j = 0; j < nblk; ++j) {
+                const int row = batch * p.Lk + j * BKV;
+                for (int c = 0; c < NCH; ++c) push(&tmK, qk_col + c * 64, row);
+                for (int d = 0; d < NVC; ++d) push(&tmV, v_col + d * 64, row);
             }
         }
-      }
     } else {
-        if (TILES == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-        else asm volatile("setmaxnreg.inc.sync.aligned.u32 200;");
-        // ---------------- softmax / output warps ----------------
-        const int x = (warp - 4) >> 2;                          // tile 0 (A) or 1 (B)
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;                       // query row inside the tile
-        const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-        const uint32_t tS = tmem_base + x * ATT_BN + lane_off;
-        const uint32_t tO = tmem_base + COL_O + x * ATT_D + lane_off;
-        const uint32_t tP = tmem_base + COL_P + x * 64 + lane_off;
-        uint32_t g = 0;                                         // blocks processed by this tile (barrier parities)
-        for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
-            if (x == 1 && !item_tileB(it)) continue;
-            const int head = item_head(it), batch = item_batch(it), q0 = item_q0(it);
-            float m_ref = 0.f, l_run = 0.f;
-            for (int j = 0; j < nblk; ++j, ++g) {
-                mbar_wait(&s_full[x], g & 1);
-                tc_fence_after();
-                uint32_t s[128];
-                tmem_ld_32x32_at<0>(tS + 0, s);
-                tmem_ld_32x32_at<32>(tS + 32, s);
-                tmem_ld_32x32_at<64>(tS + 64, s);
-                if (NKEY > 96) tmem_ld_32x32_at<96>(tS + 96, s);
-                tmem_ld_wait();
-                const int kv_valid = min(ATT_BN, p.Lk - j * ATT_BN);
-                if (kv_valid < NKEY) {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        const int wg = (warp - 4) >> 2;                              // query rows [64 wg, 64 wg + 64) of the CTA
+        const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // fragment rows r_lo and r_lo + 8
+        const int cq = 2 * (lane & 3);
+        int slot = 0;
+        uint32_t phase = 0;
+        float o[NVC][32];
 #pragma unroll
-                    for (int i = 0; i < NKEY; ++i)
-                        if (i >= kv_valid) s[i] = 0xff800000u;   // -inf
-                }
-                // row maximum with 8 independent chains (FMNMX3 pairs them up); a single chain would serialise
-                float mxa[8];
+        for (int d = 0; d < NVC; ++d)
 #pragma unroll
-                for (int t = 0; t < 8; ++t) mxa[t] = __uint_as_float(s[t]);
-#pragma unroll
-                for (int i = 8; i < NKEY; i += 8) {
-#pragma unroll
-                    for (int t = 0; t < 8; ++t) mxa[t] = fmaxf(mxa[t], __uint_as_float(s[i + t]));
-                }
-                float mx = fmaxf(fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3])),
-                                 fmaxf(fmaxf(mxa[4], mxa[5]), fmaxf(mxa[6], mxa[7])));
-                mx *= p.scale_log2;
-                // the previous PV of this tile (possibly the previous item's last) reads P, which is about to be overwritten,
-                // and updates O, which a rescale would touch
-                if (g > 0) {
-                    mbar_wait(&pv_done[x], (g - 1) & 1);
-                    tc_fence_after();
-                }
-                if (j == 0) {
-                    m_ref = mx;
-                } else {
-                    const bool need = mx > m_ref + ATT_RESCALE_THRESHOLD;
-                    if (__any_sync(0xffffffffu, need)) {
-                        const float alpha = need ? ex2_approx(m_ref - mx) : 1.0f;
-                        if (need) m_ref = mx;
-                        l_run *= alpha;
-#pragma unroll
-                        for (int c0 = 0; c0 < ATT_D; c0 += 32) {
-                            uint32_t o[32];
-                            tmem_ld_32x32(tO + c0, o);
-                            tmem_ld_wait();
-#pragma unroll
-                            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                            tmem_st_32x32(tO + c0, o);
-                        }
-                        tmem_st_wait();
-                    }
-                }
-                l_run += softmax_row_to_tmem<NKEY, EMU, ICVT>(s, p.scale_log2, m_ref, tP);
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&p_full[x]);
+            for (int i = 0; i < 32; ++i) o[d][i] = 0.f;
+        float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+        mbar_wait(q_full, 0);
+        for (int j = 0; j < nblk; ++j) {
+            // ---- S = Q K_j^T ----
+            float s[BKV / 2];
+            const int first_slot = slot;
+            {
+                int sl = slot;
+                uint32_t ph = phase;
+                for (int c = 0; c < NCH; ++c) { mbar_wait(&slot_full[sl], ph); if (++sl == SLOTS) { sl = 0; ph ^= 1; } }
             }
-            // epilogue of the item: O / l. The next item's first QK for this tile is already in flight.
-            mbar_wait(&pv_done[x], (g - 1) & 1);
-            tc_fence_after();
-            const int qrow = q0 + x * ATT_BM + row;
-            const float inv = 1.f / l_run;
-            __nv_bfloat16* dst = p.out + ((long long)batch * p.Lq + qrow) * p.ldo + head * ATT_D;
+            wgmma_fence();
 #pragma unroll
-            for (int c0 = 0; c0 < ATT_D; c0 += 32) {
-                uint32_t o[32];
-                tmem_ld_32x32(tO + c0, o);
-                tmem_ld_wait();
-                if (qrow < p.Lq) {
+            for (int c = 0; c < NCH; ++c) {
+                const uint32_t qa = smem_u32(sQ + c * SM::Q_CHUNK + wg * 64 * 128);
+                const uint32_t ka = smem_u32(ring + slot * SM::SLOT);
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        uint4 u;
-                        u.x = pack_bf16x2(__uint_as_float(o[q * 8 + 0]) * inv, __uint_as_float(o[q * 8 + 1]) * inv);
-                        u.y = pack_bf16x2(__uint_as_float(o[q * 8 + 2]) * inv, __uint_as_float(o[q * 8 + 3]) * inv);
-                        u.z = pack_bf16x2(__uint_as_float(o[q * 8 + 4]) * inv, __uint_as_float(o[q * 8 + 5]) * inv);
-                        u.w = pack_bf16x2(__uint_as_float(o[q * 8 + 6]) * inv, __uint_as_float(o[q * 8 + 7]) * inv);
-                        reinterpret_cast<uint4*>(dst + c0)[q] = u;
-                    }
+                for (int kk = 0; kk < 4; ++kk)
+                    wgmma_qk<BKV>(s, wgmma_desc_sw128(qa + 32 * kk), wgmma_desc_sw128(ka + 32 * kk), (c | kk) != 0);
+                if (++slot == SLOTS) { slot = 0; phase ^= 1; }
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_operands(s);
+            __syncwarp();
+            if (lane == 0)
+                for (int c = 0, sl = first_slot; c < NCH; ++c, sl = (sl + 1 == SLOTS ? 0 : sl + 1)) mbar_arrive(&slot_empty[sl]);
+
+            // ---- online softmax on the fragment: element 4 t + 2 h + e = row r_lo + 8 h, key 8 t + cq + e ----
+            const int kv_valid = min(BKV, p.Lk - j * BKV);
+            if (kv_valid < BKV) {
+#pragma unroll
+                for (int t = 0; t < BKV / 8; ++t)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e)
+                        if (8 * t + cq + (e & 1) >= kv_valid) s[4 * t + e] = -INFINITY;
+            }
+            float alpha[2], negm[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float mx = -INFINITY;
+#pragma unroll
+                for (int t = 0; t < BKV / 8; ++t) mx = fmaxf(mx, fmaxf(s[4 * t + 2 * h], s[4 * t + 2 * h + 1]));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                const float m_new = fmaxf(m_run[h], mx * p.scale_log2);     // every block holds >= 1 valid key: finite
+                alpha[h] = ex2_approx(m_run[h] - m_new);                    // 0 on the first block
+                m_run[h] = m_new;
+                negm[h] = -m_new;
+                l_run[h] *= alpha[h];
+            }
+#pragma unroll
+            for (int d = 0; d < NVC; ++d)
+#pragma unroll
+                for (int i = 0; i < 32; ++i) o[d][i] *= alpha[(i >> 1) & 1];
+            uint32_t pa[BKV / 16][4];                                       // P as m64k16 A fragments, one per 16 keys
+#pragma unroll
+            for (int t = 0; t < BKV / 8; ++t) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float x0 = fmaf(s[4 * t + 2 * h], p.scale_log2, negm[h]);
+                    const float x1 = fmaf(s[4 * t + 2 * h + 1], p.scale_log2, negm[h]);
+                    const int q = (2 * t + h) & 3;                          // pair index inside a group of 4
+                    const bool emulate = (EMU == 4) || (EMU == 3 && q != 1) || (EMU == 2 && (q & 1)) || (EMU == 1 && q == 3);
+                    const float e0 = emulate ? ex2_emulated(x0) : ex2_approx(x0);
+                    const float e1 = emulate ? ex2_emulated(x1) : ex2_approx(x1);
+                    l_run[h] += e0 + e1;
+                    const bool alu_pack = (ICVT == 4) || (ICVT == 2 && !(q & 1)) || (ICVT == 1 && q == 0) || (ICVT == 3 && q != 2);
+                    // A fragment of k-step t/2: regs {0, 1} = keys [0, 8) of the step for rows r, r + 8; {2, 3} = keys [8, 16)
+                    pa[t >> 1][(t & 1) * 2 + h] = alu_pack ? pack_bf16x2_alu(e0, e1) : pack_bf16x2(e0, e1);
                 }
             }
-            // O of this tile is read: order the TMEM loads before the P write / arrive that lets the next item's PV overwrite it
-            tc_fence_before();
+
+            // ---- O += P V_j ----
+            const int v_first = slot;
+            {
+                int sl = slot;
+                uint32_t ph = phase;
+                for (int d = 0; d < NVC; ++d) { mbar_wait(&slot_full[sl], ph); if (++sl == SLOTS) { sl = 0; ph ^= 1; } }
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int d = 0; d < NVC; ++d) {
+                const uint32_t va = smem_u32(ring + slot * SM::SLOT);
+#pragma unroll
+                for (int kk = 0; kk < BKV / 16; ++kk)      // 16 keys = 16 rows of 128 B = two 8-row swizzle atoms
+                    wgmma_rs_n64_tb(o[d], pa[kk], wgmma_desc_sw128(va + kk * 2048), 1);
+                if (++slot == SLOTS) { slot = 0; phase ^= 1; }
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int d = 0; d < NVC; ++d) wgmma_fence_operands(o[d]);
+            __syncwarp();
+            if (lane == 0)
+                for (int d = 0, sl = v_first; d < NVC; ++d, sl = (sl + 1 == SLOTS ? 0 : sl + 1)) mbar_arrive(&slot_empty[sl]);
+        }
+
+        // ---- O / l -> bf16 ----
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float l = l_run[h];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            const float inv = 1.f / l;
+            const int qrow = q0 + r_lo + 8 * h;
+            if (qrow < p.Lq) {
+                __nv_bfloat16* dst = p.out + ((long long)batch * p.Lq + qrow) * p.ldo + v_col + cq;
+#pragma unroll
+                for (int d = 0; d < NVC; ++d)
+#pragma unroll
+                    for (int t = 0; t < 8; ++t)
+                        *reinterpret_cast<uint32_t*>(dst + d * 64 + 8 * t) =
+                            pack_bf16x2(o[d][4 * t + 2 * h] * inv, o[d][4 * t + 2 * h + 1] * inv);
+            }
         }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
-    }
 }
 
-static long long g_att_desc_override = -1;
-static long long g_att_idesc_pv_override = -1;
 static int g_att_emu = -1;            // emulated exponent pairs per 4: -1 = environment / default
-
-static int g_att_stagger = -1;        // cycles; -1 = environment / default
-static int attention_stagger() {
-    if (g_att_stagger < 0) {
-        const char* e = getenv("SUPIR_B200_ATTN_STAGGER");
-        g_att_stagger = e ? atoi(e) : 0;
-        if (g_att_stagger < 0) g_att_stagger = 0;
-    }
-    return g_att_stagger;
-}
-
 static int g_att_icvt = -1;           // pairs of every 4 packed to bf16 on the ALU pipe: -1 = environment / default
+
 static int attention_int_pack() {
     if (g_att_icvt < 0) {
         const char* e = getenv("SUPIR_B200_ATTN_ALU_PACK");
@@ -454,72 +280,48 @@ static int attention_int_pack() {
 static int attention_emu() {
     if (g_att_emu < 0) {
         const char* e = getenv("SUPIR_B200_ATTN_EMU");
-        // default 0: on B200 the emulated pairs measured SLOWER than MUFU (profiles/r02_selftest_attnperf2.log: 817 / 808 / 740 /
-        // 652 / 568 TFLOP/s at 4096 tokens for 0..4 of 4 pairs) — the packed FFMA2 / FADD2 chain costs more issue and FMA-pipe
-        // time than the 16 MUFU cycles per pair it saves
         g_att_emu = e ? atoi(e) : 0;
         if (g_att_emu < 0 || g_att_emu > 4) g_att_emu = 0;
     }
     return g_att_emu;
 }
 
-template <int TILES, int STAGES, int NKEY, int EMU, int ICVT>
-static int launch_attention(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, AttnParams p, int B,
-                            cudaStream_t st) {
-    using S = AttnSmem<TILES, STAGES>;
-    // function attributes are per device: set them once for every device this process launches on
+template <int NCH, int NVC, int BKV, int EMU, int ICVT>
+static int launch_attention(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const AttnParams& p,
+                            int heads, int B, cudaStream_t st) {
+    using SM = AttnSmem<NCH, NVC, BKV>;
     static bool attr_set[64] = {};
-    int dev = 0;
-    SUPIR_CHECK_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(attention_d64_kernel<TILES, STAGES, NKEY, EMU, ICVT>,
-                                              cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-        if (dev >= 0 && dev < 64) attr_set[dev] = true;
+    const int dslot = current_device_slot();
+    if (!attr_set[dslot]) {
+        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel<NCH, NVC, BKV, EMU, ICVT>,
+                                              cudaFuncAttributeMaxDynamicSharedMemorySize, SM::TOTAL));
+        attr_set[dslot] = true;
     }
-    p.nqb = (p.Lq + TILES * ATT_BM - 1) / (TILES * ATT_BM);
-    p.num_items = p.nqb * p.H * B;
-    p.idesc_qk = umma_idesc_bf16(ATT_BM, NKEY, 0, 0);
-    p.stagger = TILES == 2 ? attention_stagger() : 0;
-    const int slots = device_sm_count() * (TILES == 1 ? 2 : 1);
-    const int grid = p.num_items < slots ? p.num_items : slots;
-    attention_d64_kernel<TILES, STAGES, NKEY, EMU, ICVT><<<grid, 128 + 128 * TILES, S::TOTAL, st>>>(tmQ, tmK, tmV, p);
+    const dim3 grid((p.Lq + ATT_BM - 1) / ATT_BM, heads * p.nsplit, B);
+    attention_wgmma_kernel<NCH, NVC, BKV, EMU, ICVT><<<grid, ATT_THREADS, SM::TOTAL, st>>>(tmQ, tmK, tmV, p);
     count_launch();
     SUPIR_CHECK_CUDA(cudaGetLastError());
     return SUPIR_OK;
 }
 
-template <int TILES, int STAGES, int NKEY>
-static int launch_attention_emu(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const AttnParams& p, int B,
-                                cudaStream_t st) {
-    const int emu = attention_emu(), icvt = attention_int_pack();
-    if (emu >= 2) {      // the (measured slower) exponent emulation keeps one instantiation for the record
-        return launch_attention<TILES, STAGES, NKEY, 2, 0>(tmQ, tmK, tmV, p, B, st);
-    }
-    switch (icvt) {
-        case 0: return launch_attention<TILES, STAGES, NKEY, 0, 0>(tmQ, tmK, tmV, p, B, st);
-        case 1: case 2: return launch_attention<TILES, STAGES, NKEY, 0, 2>(tmQ, tmK, tmV, p, B, st);
-        case 3: return launch_attention<TILES, STAGES, NKEY, 0, 3>(tmQ, tmK, tmV, p, B, st);
-        default: return launch_attention<TILES, STAGES, NKEY, 0, 4>(tmQ, tmK, tmV, p, B, st);
-    }
+static int make_attention_maps(CUtensorMap* tmQ, CUtensorMap* tmK, CUtensorMap* tmV, const void* q, long long ldq, const void* k,
+                               long long ldk, const void* v, long long ldv, uint64_t cols, uint64_t rows_q, uint64_t rows_kv,
+                               uint32_t bkv) {
+    int rc;
+    const uint32_t box_q[2] = {64, ATT_BM}, box_kv[2] = {64, bkv};
+    const uint64_t dq[2] = {cols, rows_q}, dkv[2] = {cols, rows_kv};
+    const uint64_t sq[1] = {(uint64_t)ldq}, sk[1] = {(uint64_t)ldk}, sv[1] = {(uint64_t)ldv};
+    if ((rc = make_tmap_bf16(tmQ, q, 2, dq, sq, box_q))) return rc;
+    if ((rc = make_tmap_bf16(tmK, k, 2, dkv, sk, box_kv))) return rc;
+    return make_tmap_bf16(tmV, v, 2, dkv, sv, box_kv);
 }
 
 }  // namespace supir
 
 using namespace supir;
 
-extern "C" int supir_debug_set_attention_descriptors(long long smem_desc_template, long long idesc_pv) {
-    g_att_desc_override = smem_desc_template;
-    g_att_idesc_pv_override = idesc_pv;
-    return SUPIR_OK;
-}
-
 extern "C" int supir_set_attention_alu_pack(int pairs_of_4) {
     g_att_icvt = pairs_of_4 < 0 ? -1 : (pairs_of_4 > 4 ? 4 : pairs_of_4);
-    return SUPIR_OK;
-}
-
-extern "C" int supir_set_attention_stagger(int cycles) {
-    g_att_stagger = cycles < 0 ? -1 : cycles;
     return SUPIR_OK;
 }
 
@@ -536,307 +338,25 @@ extern "C" int supir_attention_bf16(const void* q, long long ldq, const void* k,
     SUPIR_REQUIRE(B > 0 && H > 0 && Lq > 0 && Lk > 0, "supir_attention_bf16: bad shape");
     SUPIR_REQUIRE(scale > 0.f, "supir_attention_bf16: scale must be positive");
     SUPIR_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0, "supir_attention_bf16: leading dims must be multiples of 8");
-    const bool short_keys = Lk <= 96;          // 77-token text context: 96 key columns per block instead of 128
     CUtensorMap tmQ, tmK, tmV;
-    int rc;
-    {
-        const uint32_t box[2] = {ATT_D, ATT_BM};
-        const uint64_t dims[2] = {(uint64_t)H * ATT_D, (uint64_t)B * Lq};
-        const uint64_t str[1] = {(uint64_t)ldq};
-        if ((rc = make_tmap_bf16(&tmQ, q, 2, dims, str, box))) return rc;
-    }
-    {
-        const uint32_t box[2] = {ATT_D, (uint32_t)(short_keys ? 96 : ATT_BN)};
-        const uint64_t dims[2] = {(uint64_t)H * ATT_D, (uint64_t)B * Lk};
-        const uint64_t str[1] = {(uint64_t)ldk};
-        if ((rc = make_tmap_bf16(&tmK, k, 2, dims, str, box))) return rc;
-        const uint64_t strv[1] = {(uint64_t)ldv};
-        if ((rc = make_tmap_bf16(&tmV, v, 2, dims, strv, box))) return rc;
-    }
+    int rc = make_attention_maps(&tmQ, &tmK, &tmV, q, ldq, k, ldk, v, ldv, (uint64_t)H * 64, (uint64_t)B * Lq, (uint64_t)B * Lk, 128);
+    if (rc) return rc;
     AttnParams p{};
-    p.Lq = Lq; p.Lk = Lk; p.H = H;
+    p.Lq = Lq; p.Lk = Lk;
+    p.nsplit = 1;
+    p.head_cols = 64;
     p.ldo = ldo;
     p.out = reinterpret_cast<__nv_bfloat16*>(out);
     p.scale_log2 = scale * 1.4426950408889634f;
-    const uint64_t dt = g_att_desc_override >= 0 ? (uint64_t)g_att_desc_override
-                                                 : (((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61));
-    p.desc_hi = (uint32_t)(dt >> 32);
-    p.idesc_pv = g_att_idesc_pv_override >= 0 ? (uint32_t)g_att_idesc_pv_override : umma_idesc_bf16(ATT_BM, ATT_D, 0, 1);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    // one key block (77-token cross-attention, small ZeroCrossAttn contexts): light one-tile CTAs, two per SM, so one CTA's
-    // load / store latency hides behind the other's math; longer keys: two tiles ping-pong inside one CTA per SM.
-    if (short_keys) return launch_attention_emu<1, 2, 96>(tmQ, tmK, tmV, p, B, st);
-    if (Lk <= ATT_BN) return launch_attention_emu<1, 2, 128>(tmQ, tmK, tmV, p, B, st);
-    return launch_attention_emu<2, 4, 128>(tmQ, tmK, tmV, p, B, st);
-}
-
-// =====================================================================================================================
-// Single-head attention with head_dim 512: the SDXL VAE's mid-block AttnBlock (sgm/modules/diffusionmodules/model.py:
-// 158-206 / MemoryEfficientAttnBlock :209-262; per tile in SUPIR/utils/tilevae.py:292-336): softmax(q k^T / sqrt(512)) v over
-// ALL pixels of a (tile's) 8x-downsampled feature map (18 496 tokens for a 1088-px encoder tile, 22 500 for a 150-latent
-// decoder tile). Flash-style: the score matrix never leaves the SM (round 1 wrote it to HBM in fp32: 1.4 GB per tile).
-//
-// The 512-wide output does not fit TMEM next to S (512 fp32 columns = all of it), so a CTA owns 128 queries and ONE HALF of
-// the value columns (grid.y = 2): O[128 x 256] in TMEM columns [0, 256), two S buffers [256, 384) / [384, 512); the bf16
-// probabilities overwrite the first 64 columns of the S buffer they came from (P aliases S), so QK of block j+1 runs on the
-// tensor pipe while the softmax warps work on block j. QK^T is recomputed by both halves (1.5x the minimal FLOPs) — cheaper
-// than moving S between SMs. Q (128 x 512 bf16 = 128 KB) stays resident in shared memory as 8 K-major 64-column chunks;
-// K and V stream through one ring of 16 KB slots: 8 K chunks (64 of the 512 depth each) and 4 V chunks (64 value columns each,
-// MN-major B operand straight from the [token, channel] layout) per 128-key block, in the order the MMA thread consumes them.
-// 256 threads: warp 0 TMA producer, warp 1 MMA issuer, warps 4..7 softmax (one query row per thread), same packed-fp32 /
-// partial-emulation exponential and lazy rescale as the head_dim-64 kernel.
-// =====================================================================================================================
-namespace supir {
-
-static constexpr int A5_SLOTS = 5;
-
-// D = head dim (512 for the SDXL VAE; 128 / 256 serve the reduced-width VAE configurations of the golden fixtures):
-// D / 64 depth chunks per QK, min(D, 256) value columns per CTA.
-template <int D>
-struct Attn512Smem {
-    static constexpr int NCH = D / 64;                            // 64-wide depth chunks of Q / K
-    static constexpr int DV = D > 256 ? 256 : D;                  // value columns owned by one CTA
-    static constexpr int CHUNK = ATT_BM * 64 * 2;                 // 16 KB: 128 rows x 64 bf16
-    static constexpr int OFF_Q = 0;                               // NCH chunks
-    static constexpr int OFF_RING = OFF_Q + NCH * CHUNK;
-    static constexpr int OFF_BAR = OFF_RING + A5_SLOTS * CHUNK;
-    static constexpr int TOTAL = OFF_BAR + 256 + 1024;
-};
-
-struct Attn512Params {
-    int L;
-    long long ldo;
-    __nv_bfloat16* out;
-    float scale_log2;
-    uint32_t desc_hi, idesc_qk, idesc_pv;
-};
-
-template <int D, int EMU>
-__global__ void __launch_bounds__(256, 1)
-attention_d512_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                      const __grid_constant__ CUtensorMap tmV, const Attn512Params p) {
-    using SM = Attn512Smem<D>;
-    constexpr int NCH = SM::NCH, A5_DV = SM::DV, NVC = SM::DV / 64;
-    constexpr uint32_t COL_S = 256;                                // S buffer b at columns COL_S + 128 b
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sQ = smem + SM::OFF_Q;
-    uint8_t* ring = smem + SM::OFF_RING;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::OFF_BAR);
-    uint64_t* q_full = bars;                            // 1
-    uint64_t* slot_full = bars + 1;                     // [A5_SLOTS]
-    uint64_t* slot_empty = slot_full + A5_SLOTS;        // [A5_SLOTS]
-    uint64_t* s_full = slot_empty + A5_SLOTS;           // [2] per S buffer
-    uint64_t* p_full = s_full + 2;                      // [2]
-    // PV(j) commits pv_done[j & 1]. Two barriers because the softmax warps wait on PV only when they rescale O and at the
-    // very end: with ONE barrier flipping every block, a waiter two blocks behind would mistake an older phase for the one
-    // it wants (mbarrier waits carry one parity bit). Per parity of j the waiter is at most one phase behind: PV(j-3) has
-    // retired before S(j) could be delivered, and PV(j+1) cannot start before P(j+1) exists.
-    uint64_t* pv_done = p_full + 2;                     // [2]
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(pv_done + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int q0 = blockIdx.x * ATT_BM, half = blockIdx.y, batch = blockIdx.z;
-    const int nblk = (p.L + ATT_BN - 1) / ATT_BN;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmQ);
-        tma_prefetch_desc(&tmK);
-        tma_prefetch_desc(&tmV);
-        mbar_init(q_full, 1);
-        for (int s = 0; s < A5_SLOTS; ++s) { mbar_init(&slot_full[s], 1); mbar_init(&slot_empty[s], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&p_full[i], 4); mbar_init(&pv_done[i], 1); }
-        fence_barrier_init();
-    }
-    if (warp == 1) {
-        tmem_alloc(tmem_ptr, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-
-    if (warp < 4) {
-      // (no setmaxnreg here: 256 threads at one CTA per SM can have 255 registers each as launched)
-      if (warp == 0) {
-        if (lane == 0) {
-            // ---------------- TMA producer: Q once; then the ring in consumption order K(0), [K(j+1), V(j)]... ----------------
-            mbar_expect_tx(q_full, NCH * SM::CHUNK);
-            for (int c = 0; c < NCH; ++c) tma_load_2d(sQ + c * SM::CHUNK, &tmQ, q_full, c * 64, batch * p.L + q0);
-            int slot = 0;
-            uint32_t phase = 0;
-            auto push = [&](const CUtensorMap* tm, int col, int row) {
-                mbar_wait(&slot_empty[slot], phase ^ 1);
-                mbar_expect_tx(&slot_full[slot], SM::CHUNK);
-                tma_load_2d(ring + slot * SM::CHUNK, tm, &slot_full[slot], col, row);
-                if (++slot == A5_SLOTS) { slot = 0; phase ^= 1; }
-            };
-            for (int c = 0; c < NCH; ++c) push(&tmK, c * 64, batch * p.L);
-            for (int j = 0; j < nblk; ++j) {
-                if (j + 1 < nblk)
-                    for (int c = 0; c < NCH; ++c) push(&tmK, c * 64, batch * p.L + (j + 1) * ATT_BN);
-                for (int d = 0; d < NVC; ++d) push(&tmV, half * A5_DV + d * 64, batch * p.L + j * ATT_BN);
-            }
-        }
-      } else if (warp == 1) {
-        if (lane == 0) {
-            // ---------------- MMA issuer ----------------
-            const uint64_t dtemplate = (uint64_t)p.desc_hi << 32;
-            int slot = 0;
-            uint32_t phase = 0;
-            auto next_slot = [&]() { if (++slot == A5_SLOTS) { slot = 0; phase ^= 1; } };
-            auto issue_qk = [&](int buf) {
-                for (int c = 0; c < NCH; ++c) {
-                    mbar_wait(&slot_full[slot], phase);
-                    tc_fence_after();
-                    const uint64_t qdesc = dtemplate | ((smem_u32(sQ + c * SM::CHUNK) >> 4) & 0x3FFF);
-                    const uint64_t kdesc = dtemplate | ((smem_u32(ring + slot * SM::CHUNK) >> 4) & 0x3FFF);
-#pragma unroll
-                    for (int kk = 0; kk < 4; ++kk)
-                        umma_bf16(tmem_base + COL_S + buf * ATT_BN, qdesc + 2 * kk, kdesc + 2 * kk, p.idesc_qk, (c | kk) != 0);
-                    umma_commit(&slot_empty[slot]);
-                    next_slot();
-                }
-                umma_commit(&s_full[buf]);
-            };
-            mbar_wait(q_full, 0);
-            issue_qk(0);
-            for (int j = 0; j < nblk; ++j) {
-                const int buf = j & 1;
-                if (j + 1 < nblk) issue_qk(buf ^ 1);              // S[buf^1] is free: PV(j-1), which read P there, was issued before
-                mbar_wait(&p_full[buf], (j >> 1) & 1);            // P(j) written over S[buf]
-                tc_fence_after();
-                for (int d = 0; d < NVC; ++d) {
-                    mbar_wait(&slot_full[slot], phase);
-                    tc_fence_after();
-                    const uint32_t vbase = smem_u32(ring + slot * SM::CHUNK);
-#pragma unroll
-                    for (int kk = 0; kk < ATT_BN / 16; ++kk) {
-                        const uint32_t va = vbase + kk * 16 * 128;
-                        umma_bf16_ts(tmem_base + d * 64, tmem_base + COL_S + buf * ATT_BN + kk * 8, dtemplate | ((va >> 4) & 0x3FFF),
-                                     p.idesc_pv, (j | kk) != 0);
-                    }
-                    umma_commit(&slot_empty[slot]);
-                    next_slot();
-                }
-                umma_commit(&pv_done[buf]);
-            }
-        }
-      }
-    } else {
-        // ---------------- softmax / output warps (warps 4..7) ----------------
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;
-        const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-        const uint32_t tO = tmem_base + lane_off;
-        float m_ref = 0.f, l_run = 0.f;
-        for (int j = 0; j < nblk; ++j) {
-            const int buf = j & 1;
-            const uint32_t tS = tmem_base + COL_S + buf * ATT_BN + lane_off;
-            mbar_wait(&s_full[buf], (j >> 1) & 1);
-            tc_fence_after();
-            uint32_t s[128];
-            tmem_ld_32x32_at<0>(tS + 0, s);
-            tmem_ld_32x32_at<32>(tS + 32, s);
-            tmem_ld_32x32_at<64>(tS + 64, s);
-            tmem_ld_32x32_at<96>(tS + 96, s);
-            tmem_ld_wait();
-            const int kv_valid = min(ATT_BN, p.L - j * ATT_BN);
-            if (kv_valid < ATT_BN) {
-#pragma unroll
-                for (int i = 0; i < ATT_BN; ++i)
-                    if (i >= kv_valid) s[i] = 0xff800000u;
-            }
-            float mxa[8];
-#pragma unroll
-            for (int t = 0; t < 8; ++t) mxa[t] = __uint_as_float(s[t]);
-#pragma unroll
-            for (int i = 8; i < ATT_BN; i += 8) {
-#pragma unroll
-                for (int t = 0; t < 8; ++t) mxa[t] = fmaxf(mxa[t], __uint_as_float(s[i + t]));
-            }
-            float mx = fmaxf(fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3])), fmaxf(fmaxf(mxa[4], mxa[5]), fmaxf(mxa[6], mxa[7])));
-            mx *= p.scale_log2;
-            if (j == 0) {
-                m_ref = mx;
-            } else {
-                const bool need = mx > m_ref + ATT_RESCALE_THRESHOLD;
-                if (__any_sync(0xffffffffu, need)) {
-                    mbar_wait(&pv_done[(j - 1) & 1], ((j - 1) >> 1) & 1);   // PV(j-1) is the last writer of O
-                    tc_fence_after();
-                    const float alpha = need ? ex2_approx(m_ref - mx) : 1.0f;
-                    if (need) m_ref = mx;
-                    l_run *= alpha;
-#pragma unroll 1
-                    for (int c0 = 0; c0 < A5_DV; c0 += 32) {
-                        uint32_t o[32];
-                        tmem_ld_32x32(tO + c0, o);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                        tmem_st_32x32(tO + c0, o);
-                    }
-                    tmem_st_wait();
-                }
-            }
-            // P(j) overwrites the first 64 columns of S[buf]: its previous reader, PV(j-2), retired before QK(j) could run
-            l_run += softmax_row_to_tmem<ATT_BN, EMU, 0>(s, p.scale_log2, m_ref, tS);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&p_full[buf]);
-        }
-        mbar_wait(&pv_done[(nblk - 1) & 1], ((nblk - 1) >> 1) & 1);
-        tc_fence_after();
-        const int qrow = q0 + row;
-        const float inv = 1.f / l_run;
-        __nv_bfloat16* dst = p.out + ((long long)batch * p.L + qrow) * p.ldo + half * A5_DV;
-#pragma unroll 1
-        for (int c0 = 0; c0 < A5_DV; c0 += 32) {
-            uint32_t o[32];
-            tmem_ld_32x32(tO + c0, o);
-            tmem_ld_wait();
-            if (qrow < p.L) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    uint4 u;
-                    u.x = pack_bf16x2(__uint_as_float(o[q * 8 + 0]) * inv, __uint_as_float(o[q * 8 + 1]) * inv);
-                    u.y = pack_bf16x2(__uint_as_float(o[q * 8 + 2]) * inv, __uint_as_float(o[q * 8 + 3]) * inv);
-                    u.z = pack_bf16x2(__uint_as_float(o[q * 8 + 4]) * inv, __uint_as_float(o[q * 8 + 5]) * inv);
-                    u.w = pack_bf16x2(__uint_as_float(o[q * 8 + 6]) * inv, __uint_as_float(o[q * 8 + 7]) * inv);
-                    reinterpret_cast<uint4*>(dst + c0)[q] = u;
-                }
-            }
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
+    if (attention_emu() >= 2) return launch_attention<1, 1, 128, 2, 0>(tmQ, tmK, tmV, p, H, B, st);
+    switch (attention_int_pack()) {
+        case 0: return launch_attention<1, 1, 128, 0, 0>(tmQ, tmK, tmV, p, H, B, st);
+        case 1: case 2: return launch_attention<1, 1, 128, 0, 2>(tmQ, tmK, tmV, p, H, B, st);
+        case 3: return launch_attention<1, 1, 128, 0, 3>(tmQ, tmK, tmV, p, H, B, st);
+        default: return launch_attention<1, 1, 128, 0, 4>(tmQ, tmK, tmV, p, H, B, st);
     }
 }
-
-template <int D, int EMU>
-static int launch_attention_d512(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const Attn512Params& p,
-                                 int B, cudaStream_t st) {
-    using SM = Attn512Smem<D>;
-    static bool attr_set[64] = {};
-    int dev = 0;
-    SUPIR_CHECK_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(attention_d512_kernel<D, EMU>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::TOTAL));
-        if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
-    dim3 grid((p.L + ATT_BM - 1) / ATT_BM, D / SM::DV, B);
-    attention_d512_kernel<D, EMU><<<grid, 256, SM::TOTAL, st>>>(tmQ, tmK, tmV, p);
-    count_launch();
-    SUPIR_CHECK_CUDA(cudaGetLastError());
-    return SUPIR_OK;
-}
-
-}  // namespace supir
 
 extern "C" int supir_attention_1head_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v,
                                           long long ldv, void* out, long long ldo, int B, int L, int head_dim, float scale,
@@ -847,30 +367,22 @@ extern "C" int supir_attention_1head_bf16(const void* q, long long ldq, const vo
     SUPIR_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && ldq >= head_dim && ldk >= head_dim && ldv >= head_dim && ldo >= head_dim,
                   "supir_attention_1head_bf16: leading dims must be multiples of 8 and >= head_dim");
     CUtensorMap tmQ, tmK, tmV;
-    int rc;
-    const uint32_t box[2] = {64, ATT_BM};
-    const uint64_t dims[2] = {(uint64_t)head_dim, (uint64_t)B * L};
-    const uint64_t sq[1] = {(uint64_t)ldq}, sk[1] = {(uint64_t)ldk}, sv[1] = {(uint64_t)ldv};
-    if ((rc = make_tmap_bf16(&tmQ, q, 2, dims, sq, box))) return rc;
-    if ((rc = make_tmap_bf16(&tmK, k, 2, dims, sk, box))) return rc;
-    if ((rc = make_tmap_bf16(&tmV, v, 2, dims, sv, box))) return rc;
-    Attn512Params p{};
-    p.L = L;
+    int rc = make_attention_maps(&tmQ, &tmK, &tmV, q, ldq, k, ldk, v, ldv, (uint64_t)head_dim, (uint64_t)B * L, (uint64_t)B * L, 64);
+    if (rc) return rc;
+    AttnParams p{};
+    p.Lq = L; p.Lk = L;
+    p.head_cols = head_dim;
+    p.nsplit = head_dim == 512 ? 2 : 1;          // at most 256 value columns (128 fp32 registers of O per thread) per CTA
     p.ldo = ldo;
     p.out = reinterpret_cast<__nv_bfloat16*>(out);
     p.scale_log2 = scale * 1.4426950408889634f;
-    const uint64_t dt = g_att_desc_override >= 0 ? (uint64_t)g_att_desc_override
-                                                 : (((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61));
-    p.desc_hi = (uint32_t)(dt >> 32);
-    p.idesc_qk = umma_idesc_bf16(ATT_BM, ATT_BN, 0, 0);
-    p.idesc_pv = umma_idesc_bf16(ATT_BM, 64, 0, 1);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int emu = attention_emu();
     if (head_dim == 512) {
-        if (emu == 2) return launch_attention_d512<512, 2>(tmQ, tmK, tmV, p, B, st);
-        if (emu == 4) return launch_attention_d512<512, 4>(tmQ, tmK, tmV, p, B, st);
-        return launch_attention_d512<512, 0>(tmQ, tmK, tmV, p, B, st);
+        if (emu == 2) return launch_attention<8, 4, 64, 2, 0>(tmQ, tmK, tmV, p, 1, B, st);
+        if (emu == 4) return launch_attention<8, 4, 64, 4, 0>(tmQ, tmK, tmV, p, 1, B, st);
+        return launch_attention<8, 4, 64, 0, 0>(tmQ, tmK, tmV, p, 1, B, st);
     }
-    if (head_dim == 256) return launch_attention_d512<256, 0>(tmQ, tmK, tmV, p, B, st);
-    return launch_attention_d512<128, 0>(tmQ, tmK, tmV, p, B, st);
+    if (head_dim == 256) return launch_attention<4, 4, 64, 0, 0>(tmQ, tmK, tmV, p, 1, B, st);
+    return launch_attention<2, 2, 64, 0, 0>(tmQ, tmK, tmV, p, 1, B, st);
 }

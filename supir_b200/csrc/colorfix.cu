@@ -179,7 +179,7 @@ extern "C" int supir_image_to_uint8_bicubic(const float* x, int C, int H, int W,
     SUPIR_REQUIRE(x && out && C > 0 && H > 0 && W > 0 && h0 > 0 && w0 > 0, "supir_image_to_uint8_bicubic: bad args");
     const long long total = (long long)h0 * w0;
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > device_sm_count() * 16LL) blocks = device_sm_count() * 16LL;
     image_to_uint8_bicubic_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
         x, C, H, W, out, h0, w0, (float)H / (float)h0, (float)W / (float)w0);
     count_launch();

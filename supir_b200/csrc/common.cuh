@@ -1,5 +1,5 @@
-// supir_b200 — sm_100a device helpers: mbarrier, TMA, tcgen05/TMEM inline-PTX wrappers.
-// Every kernel in this directory is written for B200 (sm_100a) only; there is no other target.
+// supir_b200 — sm_90a device helpers: mbarrier and TMA inline-PTX wrappers (wgmma wrappers: wgmma.cuh).
+// Every kernel in this directory is written for H100 (sm_90a) only; there is no other target.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -78,8 +78,8 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 // erf-form GELU — F.gelu default used by GEGLU (reference sgm/modules/attention.py:91):  gelu(g) = g/2 + |g|/2 * erf(|g|/sqrt2).
 // erf via Abramowitz-Stegun 7.1.26 (abs err <= 1.5e-7, far below the bf16 rounding of the result) with 1/sqrt2 folded
-// into the constants: 2 MUFU (rcp, ex2) + 7 FFMA + 4 FMUL, branch-free. libdevice erff (~40 instructions with a slow
-// path) made the GEGLU epilogue issue-bound (profiles/README.md).
+// into the constants: 2 MUFU (rcp, ex2) + 7 FFMA + 4 FMUL, branch-free, where libdevice erff takes ~40 instructions
+// with a slow path.
 __device__ __forceinline__ float gelu_erf_f(float g) {
     const float ag = fabsf(g);
     float t;
@@ -175,42 +175,6 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
         : "memory");
 }
 
-// ---- thread-block cluster / CTA-pair (cta_group::2) helpers ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA loads issued by either CTA of a pair; the transaction bytes are credited to CTA 0's mbarrier (same smem offset)
-static constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-        "[%2];" ::"r"(smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(cta)
-        : "memory");
-}
 
 // TMA stores (shared -> global, bulk async group); the issuing thread tracks completion with commit / wait_group
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
@@ -233,216 +197,10 @@ __device__ __forceinline__ void bulk_wait_group_read() {
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]; bf16 inputs, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// ---- cta_group::2 variants: one MMA spans the CTA pair (M = 256: 128 rows in each CTA's TMEM; B split across the pair) ----
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// A operand read from tensor memory (rows = TMEM lanes, two bf16 k-elements per 32-bit column), B from shared memory
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive (once all prior MMAs of this thread retire) on the mbarrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(mask)
-                 : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 consecutive fp32 columns (one row per thread of the warp)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-// same, into elements [BASE, BASE+32) of a larger register array (no address-taking, so the array stays in registers)
-template <int BASE, int N>
-__device__ __forceinline__ void tmem_ld_32x32_at(uint32_t taddr, uint32_t (&r)[N]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[BASE + 0]), "=r"(r[BASE + 1]), "=r"(r[BASE + 2]), "=r"(r[BASE + 3]), "=r"(r[BASE + 4]), "=r"(r[BASE + 5]), "=r"(r[BASE + 6]), "=r"(r[BASE + 7]), "=r"(r[BASE + 8]), "=r"(r[BASE + 9]), "=r"(r[BASE + 10]), "=r"(r[BASE + 11]), "=r"(r[BASE + 12]), "=r"(r[BASE + 13]), "=r"(r[BASE + 14]), "=r"(r[BASE + 15]), "=r"(r[BASE + 16]), "=r"(r[BASE + 17]), "=r"(r[BASE + 18]), "=r"(r[BASE + 19]), "=r"(r[BASE + 20]), "=r"(r[BASE + 21]), "=r"(r[BASE + 22]), "=r"(r[BASE + 23]), "=r"(r[BASE + 24]), "=r"(r[BASE + 25]), "=r"(r[BASE + 26]), "=r"(r[BASE + 27]), "=r"(r[BASE + 28]), "=r"(r[BASE + 29]), "=r"(r[BASE + 30]), "=r"(r[BASE + 31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM: 32 lanes x 32 consecutive fp32 columns
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-        "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
-}
-
-// ---------------------------------------------------------------------------------------------
-// packed fp32 pairs (sm_100 FFMA2 / FADD2: two fp32 operations per issue slot)
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t pack2(float lo, float hi) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-    return d;
-}
-__device__ __forceinline__ uint64_t fadd2(uint64_t a, uint64_t b) {
-    uint64_t d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-__device__ __forceinline__ uint64_t fadd2_rm(uint64_t a, uint64_t b) {   // round towards -inf
-    uint64_t d;
-    asm("add.rm.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-
-__device__ __forceinline__ uint64_t fmul2(uint64_t a, uint64_t b) {
-    uint64_t d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-    return d;
-}
-// both halves rounded to bf16 and widened back to fp32 (the value a bf16 tensor would hold)
-__device__ __forceinline__ uint64_t bf16_round2(uint64_t v) {
-    float lo, hi;
-    unpack2(v, lo, hi);
-    const uint32_t pk = pack_bf16x2(lo, hi);
-    return pack2(__uint_as_float(pk << 16), __uint_as_float(pk & 0xffff0000u));
-}
-// erf-form GELU of two values (same formulation and constants as gelu_erf_f): the polynomial and the products run as packed
-// FFMA2 / FMUL2, the two MUFU operations (rcp, ex2) per element stay scalar
-__device__ __forceinline__ uint64_t gelu_erf_f2(uint64_t g) {
-    float g0, g1;
-    unpack2(g, g0, g1);
-    const uint64_t ag = pack2(fabsf(g0), fabsf(g1));
-    float d0, d1;
-    unpack2(ffma2(pack2(0.2316418882f, 0.2316418882f), ag, pack2(1.0f, 1.0f)), d0, d1);
-    float t0, t1;
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t0) : "f"(d0));
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t1) : "f"(d1));
-    const uint64_t t = pack2(t0, t1);
-    uint64_t poly = ffma2(pack2(1.061405429f, 1.061405429f), t, pack2(-1.453152027f, -1.453152027f));
-    poly = ffma2(poly, t, pack2(1.421413741f, 1.421413741f));
-    poly = ffma2(poly, t, pack2(-0.284496736f, -0.284496736f));
-    poly = ffma2(poly, t, pack2(0.254829592f, 0.254829592f));
-    poly = fmul2(poly, t);
-    float x0, x1;
-    unpack2(fmul2(fmul2(g, g), pack2(-0.7213475204f, -0.7213475204f)), x0, x1);
-    const uint64_t e = pack2(ex2_approx(x0), ex2_approx(x1));
-    float p0, p1;
-    unpack2(poly, p0, p1);
-    const uint64_t erf_abs = ffma2(pack2(-p0, -p1), e, pack2(1.0f, 1.0f));
-    const uint64_t h = fmul2(g, pack2(0.5f, 0.5f));
-    return ffma2(fmul2(ag, pack2(0.5f, 0.5f)), erf_abs, h);
-}
-
-// ---------------------------------------------------------------------------------------------
-// UMMA descriptors (layout documented in DESIGN.md §kernels; bit positions follow the PTX ISA
-// "tcgen05 shared memory descriptor" / "instruction descriptor" tables)
-// ---------------------------------------------------------------------------------------------
-// K-major operand tile stored as rows of 128 bytes (64 bf16), 128B-swizzled (what TMA SWIZZLE_128B writes):
-//   start address >> 4 in bits [0,14); LBO (unused for swizzled K-major) bits [16,30); SBO = 1024 B (8 rows) >> 4 in
-//   bits [32,46); version = 1 in bits [46,48); layout type SWIZZLE_128B = 2 in bits [61,64).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes = 1024,
-                                                   uint32_t lbo_bytes = 0) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// instruction descriptor for kind::f16 with bf16 A/B and fp32 accumulate
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major = 0, int b_mn_major = 0) {
-    return (1u << 4)                       // c_format = F32
-           | (1u << 7)                     // a_format = BF16
-           | (1u << 10)                    // b_format = BF16
-           | ((uint32_t)a_mn_major << 15)  // a_major
-           | ((uint32_t)b_mn_major << 16)  // b_major
-           | ((uint32_t)(N >> 3) << 17)    // n_dim
-           | ((uint32_t)(M >> 4) << 24);   // m_dim
 }
 
 }  // namespace supir

@@ -6,7 +6,7 @@ namespace supir {
 
 static inline unsigned blocks_for(long long n, int threads) {
     long long b = (n + threads - 1) / threads;
-    const long long cap = 148LL * 32;
+    const long long cap = device_sm_count() * 32LL;   // grid-stride loops: 32 blocks per SM
     if (b > cap) b = cap;
     if (b < 1) b = 1;
     return (unsigned)b;

@@ -1,29 +1,25 @@
-// supir_b200 — K2/K3/K4 of SURVEY.md §2a: Linear, conv1x1 and conv3x3 (implicit GEMM) on tcgen05.
+// supir_b200 — K2/K3/K4 of SURVEY.md §2a: Linear, conv1x1 and conv3x3 (implicit GEMM) on Hopper wgmma.
 //
-//   out[m, n] = epilogue( sum_k A[m, k] * W[n, k] )          bf16 x bf16 -> fp32 (TMEM) -> bf16/fp32
+//   out[m, n] = epilogue( sum_k A[m, k] * W[n, k] )          bf16 x bf16 -> fp32 (registers) -> bf16/fp32
 //
 // Replaces, on the sampling path of the reference: nn.Linear (sgm/modules/attention.py:213-218,87,106,587,611),
 // nn.Conv2d 1x1 (openaimodel.py:317, SUPIR_v0.py:48,87, model.py:124-126,164-175) and nn.Conv2d 3x3 stride 1 pad 1
 // (openaimodel.py:263,300-307; SUPIR_v0.py:79,82-83; model.py:108-117 ...).
 //
-// Design (one persistent CTA per SM, 320 threads, warp-specialised):
-//   warp 0 lane 0 : TMA producer.  A tile = 128 rows x 64 k (bf16, 128B-swizzled), W tile = BN rows x 64 k.
+// Design (one persistent CTA per SM, 384 threads = three warpgroups, warp-specialised):
+//   warpgroup 0, thread 0 : TMA producer.  A tile = 128 rows x 64 k (bf16, 128B-swizzled), W tile = BN rows x 64 k.
 //                   GEMM mode: A is a 2-D tensor map over [M, K].
 //                   CONV mode: A is a 4-D tensor map over the NHWC activation [B, H, W, C]; the tile's 128 rows are a
 //                   TH x TW pixel patch and the k-loop runs over (tap, 64-channel chunk); the tap shift is applied to the
 //                   TMA coordinates, and TMA's out-of-bounds zero fill IS the conv padding (no im2col buffer).
-//   warp 1 lane 0 : tcgen05.mma issuer (UMMA 128 x BN x 16, accumulators in TMEM, double-buffered across tiles).
-//   warps 2..9    : epilogue, two warps per TMEM lane quadrant taking alternate 32-column chunks (tcgen05.ld of the next
-//                   chunk is in flight while the current one is converted and stored); +bias, +per-batch vector (timestep embedding),
-//                   SiLU / GEGLU, bf16 round, +residual (a TMA-loaded tile), swizzled shared-memory staging and a TMA
-//                   store per chunk; a direct-store fallback serves fp32 outputs and unaligned shapes.
-// Pipelines: smem full/empty ring (TMA <-> MMA) and TMEM full/empty (MMA <-> epilogue).
-// CTAS = 2 (template parameter): the same kernel on a 2-CTA cluster, one 256 x BN tile per pair with
-// tcgen05.mma.cta_group::2 — CTA r owns rows [128 r, 128 r + 128), loads its own A tile and half of the W tile with the
-// bytes credited to CTA 0's mbarrier; CTA 0 issues the MMAs for both and multicasts the commits; the peer's epilogue warps
-// release the accumulator with a remote mbarrier arrive.
+//   warpgroups 1, 2       : wgmma consumers, rows [0, 64) and [64, 128) of the tile (m64nBNk16, fp32 accumulators in
+//                   registers, one wgmma group kept in flight); then the epilogue straight from the accumulator fragment:
+//                   +bias, +per-batch vector (timestep embedding), folded LayerNorm, SiLU / GEGLU, bf16 round, +residual,
+//                   bf16 or fp32 stores. The producer keeps filling the shared-memory ring for the next tile meanwhile.
+// Pipeline: smem full/empty mbarrier ring (TMA <-> wgmma).
 #include "common.cuh"
 #include "supir_b200.h"
+#include "wgmma.cuh"
 
 #include <cstdlib>
 #include <mutex>
@@ -32,7 +28,7 @@ namespace supir {
 
 static constexpr int BM = 128;
 static constexpr int BK = 64;
-static constexpr int GEMM_THREADS = 320;   // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two per TMEM lane quadrant)
+static constexpr int GEMM_THREADS = 384;   // warpgroup 0: TMA; warpgroups 1, 2: wgmma + epilogue (64 rows each)
 
 struct GemmKernelParams {
     int M, N, K;          // N = accumulator columns (before GEGLU halving)
@@ -58,542 +54,226 @@ struct GemmKernelParams {
     long long ldc;
     int out_f32;
     int n_out;            // valid output columns (N or N/2 for GEGLU)
-    int nimg;             // conv mode: number of images (patches beyond it are padding of the last CTA pair)
-    int staged;           // 1: epilogue through shared memory (bias tile in smem, TMA-loaded residual, TMA store)
-    int has_res;          // staged path: residual tensor map valid
+    int nimg;             // conv mode: number of images
     const float2* ln_stats;  // per-row (rstd, mean * rstd) of A: LayerNorm folded into the epilogue (see supir_epilogue), or null
     const float* ln_colsum;  // [N] row sums of the (gamma-scaled) weight matrix
-    int warp_epi;         // staged path: 1 = every epilogue warp moves ITS 32 rows with its own TMA operations (no named barriers)
-    uint32_t desc_hi;     // upper 32 bits of the shared-memory matrix descriptor (SBO / version / swizzle mode)
-    uint32_t desc_lbo;    // LBO field (bits 16..29 of the low word), pre-shifted
-    uint32_t idesc;       // tcgen05 instruction descriptor
 };
 
-template <int BN, int CTAS = 1>
+template <int BN>
 struct GemmSmem {
     static constexpr int A_BYTES = BM * BK * 2;
-    static constexpr int B_BYTES = (BN / CTAS) * BK * 2;   // a CTA pair splits the B tile
+    static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGES = CTAS == 2 ? (BN == 256 ? 4 : 6) : ((BN == 256) ? 3 : (BN == 160 ? 4 : (BN == 128 ? 4 : 6)));
-    // epilogue staging: per half-group (4 warps = 128 rows) two 8 KB output buffers and two 8 KB residual buffers
-    // (128 rows x 32 bf16 columns, 64B-swizzled), plus the tile's bias (+ per-image vector) for both accumulators
-    static constexpr int CH_BYTES = BM * 32 * 2;
-    static constexpr int EPI_BYTES = 8 * CH_BYTES + 4 * BN * 4;     // + bias and LayerNorm column-sum tiles for both accumulators
-    static constexpr int ACC_STRIDE = (BN == 160) ? 256 : BN;          // TMEM column offset of the second accumulator
-    static constexpr int TMEM_COLS = (BN == 160) ? 512 : 2 * BN;       // allocation must be a power of two
-    static constexpr int BAR_BYTES = 512;
-    static constexpr int TOTAL = STAGES * STAGE_BYTES + EPI_BYTES + BAR_BYTES + 1024;  // +1024 alignment slack
+    static constexpr int STAGES = (192 * 1024) / STAGE_BYTES > 8 ? 8 : (192 * 1024) / STAGE_BYTES;   // 4..8 stages, <= 192 KB
+    static constexpr int BAR_BYTES = 256;
+    static constexpr int TOTAL = STAGES * STAGE_BYTES + BAR_BYTES + 1024;  // +1024 alignment slack
 };
 
-template <int BN, int CTAS>
+template <int BN>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
+    if constexpr (BN == 256) wgmma_ss_n256(d, da, db, scale_d);
+    else if constexpr (BN == 160) wgmma_ss_n160(d, da, db, scale_d);
+    else if constexpr (BN == 128) wgmma_ss_n128(d, da, db, scale_d);
+    else wgmma_ss_n64(d, da, db, scale_d);
+}
+
+// two adjacent output columns (n, n + 1) of one row; `n1ok`: column n + 1 exists
+__device__ __forceinline__ void store_pair(const GemmKernelParams& p, long long grow, int n, float v0, float v1, bool n1ok) {
+    if (p.out_f32) {
+        float* dst = reinterpret_cast<float*>(p.out) + grow * p.ldc + n;
+        if (n1ok && ((reinterpret_cast<uintptr_t>(dst) & 7) == 0)) { *reinterpret_cast<float2*>(dst) = make_float2(v0, v1); }
+        else { dst[0] = v0; if (n1ok) dst[1] = v1; }
+    } else {
+        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.ldc + n;
+        if (n1ok && ((reinterpret_cast<uintptr_t>(dst) & 3) == 0)) { *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(v0, v1); }
+        else { dst[0] = __float2bfloat16_rn(v0); if (n1ok) dst[1] = __float2bfloat16_rn(v1); }
+    }
+}
+__device__ __forceinline__ float2 load_res_pair(const GemmKernelParams& p, long long grow, int n, bool n1ok) {
+    const __nv_bfloat16* src = p.residual + grow * p.ldr + n;
+    if (n1ok && ((reinterpret_cast<uintptr_t>(src) & 3) == 0)) return unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(src)));
+    return make_float2(__bfloat162float(src[0]), n1ok ? __bfloat162float(src[1]) : 0.f);
+}
+
+template <int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
-                    const GemmKernelParams p) {
-    using S = GemmSmem<BN, CTAS>;
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKernelParams p) {
+    using S = GemmSmem<BN>;
     constexpr int STAGES = S::STAGES;
-    // CTAS == 2: two CTAs of a cluster work on one 256 x BN tile (tcgen05 cta_group::2). CTA `cta_rank` owns rows
-    // [rank*128, rank*128+128) of the tile and loads its own A tile and its half of the B tile; CTA 0 issues the MMAs.
-    const uint32_t cta_rank = CTAS == 2 ? cluster_ctarank() : 0;
-    const int tile_start = CTAS == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-    const int tile_step = CTAS == 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + STAGES * S::A_BYTES;
-    uint8_t* smem_epi = smem + STAGES * S::STAGE_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_epi + S::EPI_BYTES);
-    uint64_t* full_bar = bars;                    // [STAGES]
-    uint64_t* empty_bar = bars + STAGES;          // [STAGES]
-    uint64_t* tmem_full = bars + 2 * STAGES;      // [2]
-    uint64_t* tmem_empty = bars + 2 * STAGES + 2; // [2]
-    uint64_t* res_full = bars + 2 * STAGES + 4;   // [8 epilogue warps][2 buffers] (group mode uses [2 half-groups][2 buffers])
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 20);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES);   // [STAGES]
+    uint64_t* empty_bar = full_bar + STAGES;                                              // [STAGES]
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int num_tiles = p.num_m_tiles * p.num_n_tiles;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&tmem_full[a], 1);
-            mbar_init(&tmem_empty[a], 8 * CTAS);  // one arrive per epilogue warp (of both CTAs of a pair)
-        }
-        for (int a = 0; a < 16; ++a) mbar_init(&res_full[a], 1);
-        if (p.staged) {
-            tma_prefetch_desc(&tmC);
-            if (p.has_res) tma_prefetch_desc(&tmR);
+            mbar_init(&empty_bar[s], 8);   // one arrive per consumer warp
         }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        if (CTAS == 2) { tmem_alloc_2sm(tmem_ptr, S::TMEM_COLS); tmem_relinquish_2sm(); }
-        else { tmem_alloc(tmem_ptr, S::TMEM_COLS); tmem_relinquish(); }
-    }
-    tc_fence_before();
     __syncthreads();
-    if (CTAS == 2) cluster_sync_all();     // the peer's barriers must be initialised before any remote arrive / TMA credit
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (threadIdx.x == 0) {
             // ===================== TMA producer =====================
             int stage = 0;
             uint32_t phase = 0;
-            for (int tile = tile_start; tile < num_tiles; tile += tile_step) {
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const int mt = p.m_fastest ? tile % p.num_m_tiles : tile / p.num_n_tiles;
                 const int nt = p.m_fastest ? tile / p.num_m_tiles : tile % p.num_n_tiles;
-                const int rt = mt * CTAS + (int)cta_rank;          // 128-row tile handled by this CTA
                 int b = 0, y0 = 0, x0 = 0;
                 if (p.conv) {
                     const int per_img = p.tiles_x * p.tiles_y;
-                    b = rt / per_img;
-                    const int r = rt % per_img;
+                    b = mt / per_img;
+                    const int r = mt % per_img;
                     y0 = (r / p.tiles_x) * p.TH;
                     x0 = (r % p.tiles_x) * p.TW;
                 }
-                const int bn0 = nt * BN + (int)cta_rank * (BN / CTAS);   // first W row of this CTA's share of the B tile
+                const int bn0 = nt * BN;
                 // conv mode walks (tap row, tap column, 64-channel chunk) with counters: no division in the per-k-block path
-                // (two runtime divisions per k-block cost the conv kernels 5-13 % when the geometry mode first added them)
                 int cc = 0, tx = 0, ty = 0, wcol = 0;
                 const int ax0 = x0 * p.stride + p.off_x, ay0 = y0 * p.stride + p.off_y;
                 for (int kb = 0; kb < p.num_kb; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
-                    if (CTAS == 1 || cta_rank == 0) mbar_expect_tx(&full_bar[stage], CTAS * S::STAGE_BYTES);
+                    mbar_expect_tx(&full_bar[stage], S::STAGE_BYTES);
                     uint8_t* sa = smem_a + stage * S::A_BYTES;
                     uint8_t* sb = smem_b + stage * S::B_BYTES;
                     if (p.conv) {
-                        const int ax = ax0 + tx, ay = ay0 + ty;
-                        if (CTAS == 2) {
-                            tma_load_4d_2sm(sa, &tmA, &full_bar[stage], cc * BK, ax, ay, b);
-                            tma_load_2d_2sm(sb, &tmB, &full_bar[stage], wcol + cc * BK, bn0);
-                        } else {
-                            tma_load_4d(sa, &tmA, &full_bar[stage], cc * BK, ax, ay, b);
-                            tma_load_2d(sb, &tmB, &full_bar[stage], wcol + cc * BK, bn0);
-                        }
+                        tma_load_4d(sa, &tmA, &full_bar[stage], cc * BK, ax0 + tx, ay0 + ty, b);
+                        tma_load_2d(sb, &tmB, &full_bar[stage], wcol + cc * BK, bn0);
                         if (++cc == p.kchunks) {                       // next tap: W columns advance by Cin
                             cc = 0;
                             wcol += p.Cin;
                             if (++tx == p.ntaps_x) { tx = 0; ++ty; }
                         }
                     } else {
-                        if (CTAS == 2) {
-                            tma_load_2d_2sm(sa, &tmA, &full_bar[stage], kb * BK, rt * BM);
-                            tma_load_2d_2sm(sb, &tmB, &full_bar[stage], kb * BK, bn0);
-                        } else {
-                            tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, rt * BM);
-                            tma_load_2d(sb, &tmB, &full_bar[stage], kb * BK, bn0);
-                        }
+                        tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, mt * BM);
+                        tma_load_2d(sb, &tmB, &full_bar[stage], kb * BK, bn0);
                     }
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && cta_rank == 0) {
-            // ===================== MMA issuer (CTA 0 of a pair issues for both) =====================
-            const uint32_t idesc = p.idesc;
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int tile = tile_start; tile < num_tiles; tile += tile_step) {
-                mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * S::ACC_STRIDE;
-                for (int kb = 0; kb < p.num_kb; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint64_t dtemplate = ((uint64_t)p.desc_hi << 32) | p.desc_lbo;
-                    const uint64_t adesc = dtemplate | ((smem_u32(smem_a + stage * S::A_BYTES) >> 4) & 0x3FFF);
-                    const uint64_t bdesc = dtemplate | ((smem_u32(smem_b + stage * S::B_BYTES) >> 4) & 0x3FFF);
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        // advance 16 k-elements = 32 bytes inside the 128B swizzle atom: +2 in the (addr>>4) field
-                        if (CTAS == 2) umma_bf16_2sm(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-                        else umma_bf16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0);
-                    }
-                    // smem slot free (in both CTAs of a pair) once these MMAs retire
-                    if (CTAS == 2) umma_commit_2sm(&empty_bar[stage], 3); else umma_commit(&empty_bar[stage]);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-                if (CTAS == 2) umma_commit_2sm(&tmem_full[acc], 3); else umma_commit(&tmem_full[acc]);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if (p.staged) {
-        // ===================== epilogue, staged through shared memory (warps 2..9) =====================
-        // half-group h = 4 warps = all 128 accumulator rows; it owns the 32-column chunks c = h, h+2, ... of the tile.
-        // Per chunk: TMEM -> registers (+bias, activation, +residual read from a TMA-loaded smem tile) -> bf16 -> swizzled
-        // smem -> one TMA store. Global traffic is whole lines moved by the TMA engine; the LSU only sees shared memory.
-        // warp_epi mode: every warp loads / stores ITS 32 rows of the chunk with its own TMA operations (32-row boxes) and
-        // mbarriers, so the chunk loop has no cross-warp barrier at all.
-        const int quad = warp & 3;
-        const int h = (warp - 2) >> 2;
-        const int row = quad * 32 + lane;                          // accumulator row = TMEM lane
-        const bool wl = p.warp_epi != 0;
-        const bool elected = wl ? (lane == 0) : ((warp == 2 + 4 * h) && lane == 0);
-        const int sub = wl ? quad * 32 : 0;                        // first row this thread's TMA operations cover in the chunk buffers
-        const uint32_t res_bytes = wl ? 32 * 64 : BM * 64;
-        const int epi_tid = (warp - 2) * 32 + lane;                // 0..255
-        const bool geglu = p.act == 2;
-        uint8_t* stage_c = smem_epi + h * 2 * S::CH_BYTES;
-        uint8_t* stage_r = smem_epi + 4 * S::CH_BYTES + h * 2 * S::CH_BYTES;
-        float* s_bias = reinterpret_cast<float*>(smem_epi + 8 * S::CH_BYTES);
-        float* s_c1 = s_bias + 2 * BN;
-        uint64_t* my_res_full = res_full + (wl ? 2 * (warp - 2) : 2 * h);
-        // swizzled 16-byte chunk position inside a staging row (64B swizzle for 64-byte rows, 32B swizzle for GEGLU's 32-byte rows)
-        const int row_bytes = geglu ? 32 : 64;
-        const int sw = geglu ? ((row >> 2) & 1) : ((row >> 1) & 3);
-        uint32_t cnt = 0;                                          // chunks processed by this half-group (buffer parity)
-        uint32_t res_phase[2] = {0, 0};
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        constexpr int NCH = BN / 32;
-        for (int tile = tile_start; tile < num_tiles; tile += tile_step) {
-            const int mt = p.m_fastest ? tile % p.num_m_tiles : tile / p.num_n_tiles;
-            const int nt = p.m_fastest ? tile / p.num_m_tiles : tile % p.num_n_tiles;
-            const int rt = mt * CTAS + (int)cta_rank;
-            int cb = 0, cy0 = 0, cx0 = 0;
-            if (p.conv) {
-                const int per_img = p.tiles_x * p.tiles_y;
-                cb = rt / per_img;
-                const int r = rt % per_img;
-                cy0 = (r / p.tiles_x) * p.TH;
-                cx0 = (r % p.tiles_x) * p.TW;
-            }
-            // number of chunks of this tile that hold valid columns, and how many of them are mine
-            int nvalid = (p.N - nt * BN + 31) / 32;
-            nvalid = nvalid > NCH ? NCH : nvalid;
-            const int nck = nvalid > h ? (nvalid - h + 1) / 2 : 0;
-            auto out_col = [&](int k) { const int n0 = nt * BN + (h + 2 * k) * 32; return geglu ? (n0 >> 1) : n0; };
-            // rows covered by this thread's TMA operations: the whole 128-row chunk, or (warp_epi) this warp's 32 rows =
-            // rows [rt*128 + sub, +32) of the matrix / pixels [sub, sub+32) of the TH x TW patch
-            const int sx = p.conv ? cx0 + sub % p.TW : 0, sy = p.conv ? cy0 + sub / p.TW : 0;
-            auto issue_res = [&](int k, int buf) {
-                mbar_expect_tx(&my_res_full[buf], res_bytes);
-                uint8_t* dst = stage_r + buf * S::CH_BYTES + sub * 64;
-                if (p.conv) tma_load_4d(dst, &tmR, &my_res_full[buf], out_col(k), sx, sy, cb);
-                else tma_load_2d(dst, &tmR, &my_res_full[buf], out_col(k), rt * BM + sub);
-            };
-            // tile prologue: bias (+ per-image vector) for the tile's columns; first two residual chunks
-            float* sb = s_bias + acc * BN;
-            float* sc = s_c1 + acc * BN;
-            if (epi_tid < BN) {
-                const int n = nt * BN + epi_tid;
-                float b = 0.f, c1 = 0.f;
-                if (n < p.N) {
-                    if (p.bias) b = __ldg(p.bias + n);
-                    if (p.rowvec && cb < p.nimg) b += __ldg(p.rowvec + (long long)cb * p.rowvec_ld + n);
-                    if (p.ln_colsum) c1 = __ldg(p.ln_colsum + n);
-                }
-                sb[epi_tid] = b;
-                sc[epi_tid] = c1;
-            }
-            // folded LayerNorm: out = rstd * acc - (mean * rstd) * colsum + bias', one (rstd, mean * rstd) pair per row
-            float ln_rs = 1.f, ln_nm = 0.f;
-            if (p.ln_stats) {
-                const long long grow = (long long)rt * BM + row;
-                if (grow < p.M) { const float2 st = __ldg(p.ln_stats + grow); ln_rs = st.x; ln_nm = -st.y; }
-            }
-            named_bar_sync(5, 256);
-            if (p.has_res && elected) {
-                if (nck > 0) issue_res(0, cnt & 1);
-                if (nck > 1) issue_res(1, (cnt + 1) & 1);
-            }
-            mbar_wait(&tmem_full[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t t_row = tmem_base + acc * S::ACC_STRIDE + ((uint32_t)(quad * 32) << 16);
-            uint32_t ra[32], rb[32];
-            if (nck > 0) tmem_ld_32x32(t_row + h * 32, ra);
-            auto finish = [&](uint32_t (&r)[32], int k) {
-                const int c = h + 2 * k;
-                const int buf = (cnt + k) & 1;
-                const float* bc = sb + c * 32;
-                const float* cc = sc + c * 32;
-                uint4 q[4];
-                if (geglu) {
-                    // packed fp32 pairs (FADD2 / FFMA2 / FMUL2): two outputs per issue slot outside the MUFU operations
-                    uint32_t o[8];
-#pragma unroll
-                    for (int j = 0; j < 16; j += 2) {
-                        const float2 bx = *reinterpret_cast<const float2*>(bc + j);
-                        const float2 bg = *reinterpret_cast<const float2*>(bc + 16 + j);
-                        const uint64_t xv = bf16_round2(fadd2(pack2(__uint_as_float(r[j]), __uint_as_float(r[j + 1])), pack2(bx.x, bx.y)));
-                        const uint64_t gv = bf16_round2(fadd2(pack2(__uint_as_float(r[16 + j]), __uint_as_float(r[17 + j])), pack2(bg.x, bg.y)));
-                        float o0, o1;
-                        unpack2(fmul2(xv, bf16_round2(gelu_erf_f2(gv))), o0, o1);
-                        o[j >> 1] = pack_bf16x2(o0, o1);
-                    }
-                    q[0] = make_uint4(o[0], o[1], o[2], o[3]);
-                    q[1] = make_uint4(o[4], o[5], o[6], o[7]);
-                } else {
-                    float v[32];
-                    if (p.ln_stats) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            const float4 b4 = *reinterpret_cast<const float4*>(bc + j);
-                            const float4 c4 = *reinterpret_cast<const float4*>(cc + j);
-                            v[j] = fmaf(__uint_as_float(r[j]), ln_rs, fmaf(ln_nm, c4.x, b4.x));
-                            v[j + 1] = fmaf(__uint_as_float(r[j + 1]), ln_rs, fmaf(ln_nm, c4.y, b4.y));
-                            v[j + 2] = fmaf(__uint_as_float(r[j + 2]), ln_rs, fmaf(ln_nm, c4.z, b4.z));
-                            v[j + 3] = fmaf(__uint_as_float(r[j + 3]), ln_rs, fmaf(ln_nm, c4.w, b4.w));
-                        }
-                    } else {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        const float4 b4 = *reinterpret_cast<const float4*>(bc + j);
-                        v[j] = __uint_as_float(r[j]) + b4.x;
-                        v[j + 1] = __uint_as_float(r[j + 1]) + b4.y;
-                        v[j + 2] = __uint_as_float(r[j + 2]) + b4.z;
-                        v[j + 3] = __uint_as_float(r[j + 3]) + b4.w;
-                    }
-                    }
-                    if (p.act == 1) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) v[j] = silu_f(bf16_round(v[j]));
-                    }
-                    if (p.has_res) {
-                        mbar_wait(&my_res_full[buf], res_phase[buf]);
-                        res_phase[buf] ^= 1;
-                        const uint8_t* rrow = stage_r + buf * S::CH_BYTES + row * 64;
-#pragma unroll
-                        for (int j4 = 0; j4 < 4; ++j4) {
-                            const uint4 u = *reinterpret_cast<const uint4*>(rrow + ((j4 ^ sw) << 4));
-                            const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-                            for (int t = 0; t < 4; ++t) {
-                                const float2 f = unpack_bf16x2(w[t]);
-                                v[j4 * 8 + 2 * t] = bf16_round(v[j4 * 8 + 2 * t]) + f.x;
-                                v[j4 * 8 + 2 * t + 1] = bf16_round(v[j4 * 8 + 2 * t + 1]) + f.y;
-                            }
-                        }
-                    }
-#pragma unroll
-                    for (int j4 = 0; j4 < 4; ++j4)
-                        q[j4] = make_uint4(pack_bf16x2(v[j4 * 8], v[j4 * 8 + 1]), pack_bf16x2(v[j4 * 8 + 2], v[j4 * 8 + 3]),
-                                           pack_bf16x2(v[j4 * 8 + 4], v[j4 * 8 + 5]), pack_bf16x2(v[j4 * 8 + 6], v[j4 * 8 + 7]));
-                }
-                // the TMA store issued two chunks ago read this staging buffer: make sure it is done, tell the group
-                if (elected) bulk_wait_group_read<1>();
-                if (wl) __syncwarp(); else named_bar_sync(1 + h, 128);
-                uint8_t* crow = stage_c + buf * S::CH_BYTES + row * row_bytes;
-                if (geglu) {
-                    *reinterpret_cast<uint4*>(crow + ((0 ^ sw) << 4)) = q[0];
-                    *reinterpret_cast<uint4*>(crow + ((1 ^ sw) << 4)) = q[1];
-                } else {
-#pragma unroll
-                    for (int j4 = 0; j4 < 4; ++j4) *reinterpret_cast<uint4*>(crow + ((j4 ^ sw) << 4)) = q[j4];
-                }
-                fence_proxy_async_smem();
-                if (wl) __syncwarp(); else named_bar_sync(1 + h, 128);
-                if (elected) {
-                    const uint8_t* src = stage_c + buf * S::CH_BYTES + sub * row_bytes;
-                    if (p.conv) tma_store_4d(&tmC, src, out_col(k), sx, sy, cb);
-                    else tma_store_2d(&tmC, src, out_col(k), rt * BM + sub);
-                    bulk_commit_group();
-                    if (p.has_res && k + 2 < nck) issue_res(k + 2, buf);
-                }
-            };
-#pragma unroll 1
-            for (int k = 0; k < nck; k += 2) {
-                tmem_ld_wait();
-                if (k + 1 < nck) tmem_ld_32x32(t_row + (h + 2 * (k + 1)) * 32, rb);
-                else { tc_fence_before(); __syncwarp(); if (lane == 0) { if (CTAS == 2 && cta_rank != 0) mbar_arrive_cluster(&tmem_empty[acc], 0); else mbar_arrive(&tmem_empty[acc]); } }
-                finish(ra, k);
-                if (k + 1 >= nck) break;
-                tmem_ld_wait();
-                if (k + 2 < nck) tmem_ld_32x32(t_row + (h + 2 * (k + 2)) * 32, ra);
-                else { tc_fence_before(); __syncwarp(); if (lane == 0) { if (CTAS == 2 && cta_rank != 0) mbar_arrive_cluster(&tmem_empty[acc], 0); else mbar_arrive(&tmem_empty[acc]); } }
-                finish(rb, k + 1);
-            }
-            if (nck == 0) { tc_fence_before(); __syncwarp(); if (lane == 0) { if (CTAS == 2 && cta_rank != 0) mbar_arrive_cluster(&tmem_empty[acc], 0); else mbar_arrive(&tmem_empty[acc]); } }
-            cnt += nck;
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-        if (elected) bulk_wait_group_read<0>();      // shared memory must outlive the last TMA stores
     } else {
-        // ===================== epilogue, direct global stores (fp32 output / unaligned cases; warps 2..9) =================
-        const int quad = warp & 3;  // TMEM lane quadrant this warp may access
-        const int row_in_tile = quad * 32 + lane;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int tile = tile_start; tile < num_tiles; tile += tile_step) {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        // ===================== wgmma consumers + epilogue (warpgroups 1, 2) =====================
+        const int wg = (warp - 4) >> 2;                       // rows [64 wg, 64 wg + 64) of the tile
+        const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // accumulator rows r_lo and r_lo + 8
+        const int cq = 2 * (lane & 3);                        // first of the two columns this thread holds per 8-column block
+        float acc[BN / 2];
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             const int mt = p.m_fastest ? tile % p.num_m_tiles : tile / p.num_n_tiles;
             const int nt = p.m_fastest ? tile / p.num_m_tiles : tile % p.num_n_tiles;
-            // global row / validity
-            long long grow;
-            int batch_idx;
-            bool row_ok;
-            const int rt = mt * CTAS + (int)cta_rank;
-            if (p.conv) {
-                const int per_img = p.tiles_x * p.tiles_y;
-                const int b = rt / per_img;
-                const int r = rt % per_img;
-                const int y = (r / p.tiles_x) * p.TH + row_in_tile / p.TW;
-                const int x = (r % p.tiles_x) * p.TW + row_in_tile % p.TW;
-                row_ok = (y < p.H) && (x < p.W) && (b < p.nimg);
-                grow = ((long long)b * p.out_H + (long long)y * p.out_sy + p.out_oy) * p.out_W + (long long)x * p.out_sx + p.out_ox;
-                batch_idx = b;
-            } else {
-                grow = (long long)rt * BM + row_in_tile;
-                row_ok = grow < p.M;
-                batch_idx = p.rows_per_batch > 0 ? (int)(grow / p.rows_per_batch) : 0;
+            int prev = -1;
+            for (int kb = 0; kb < p.num_kb; ++kb) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint32_t a_addr = smem_u32(smem_a + stage * S::A_BYTES + wg * 64 * 128);
+                const uint32_t b_addr = smem_u32(smem_b + stage * S::B_BYTES);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k)       // 16 k-elements = 32 bytes inside the 128B swizzle row
+                    wgmma_tile<BN>(acc, wgmma_desc_sw128(a_addr + 32 * k), wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
+                wgmma_commit();
+                wgmma_wait<1>();                         // the previous k-block's group has retired: its slot is free
+                if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
-            mbar_wait(&tmem_full[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t t_row = tmem_base + acc * S::ACC_STRIDE + ((uint32_t)(quad * 32) << 16);
-            const int half = (warp - 2) >> 2;          // this warp takes chunks half, half + 2, half + 4, ...
-            auto process = [&](uint32_t (&r)[32], int c0) {
-                const int n0 = nt * BN + c0;
-                if (row_ok) {
-                    float v[32];
+            wgmma_wait<0>();
+            wgmma_fence_operands(acc);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+            // ---------------- epilogue, from the accumulator fragment ----------------
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-                    if (p.ln_stats) {
-                        const float2 st = __ldg(p.ln_stats + grow);
+            for (int h = 0; h < 2; ++h) {
+                const int row_in_tile = r_lo + 8 * h;
+                long long grow;
+                int batch_idx;
+                bool row_ok;
+                if (p.conv) {
+                    const int per_img = p.tiles_x * p.tiles_y;
+                    const int b = mt / per_img;
+                    const int r = mt % per_img;
+                    const int y = (r / p.tiles_x) * p.TH + row_in_tile / p.TW;
+                    const int x = (r % p.tiles_x) * p.TW + row_in_tile % p.TW;
+                    row_ok = (y < p.H) && (x < p.W) && (b < p.nimg);
+                    grow = ((long long)b * p.out_H + (long long)y * p.out_sy + p.out_oy) * p.out_W + (long long)x * p.out_sx + p.out_ox;
+                    batch_idx = b;
+                } else {
+                    grow = (long long)mt * BM + row_in_tile;
+                    row_ok = grow < p.M;
+                    batch_idx = p.rows_per_batch > 0 ? (int)(grow / p.rows_per_batch) : 0;
+                }
+                if (!row_ok) continue;
+                const float* rv = p.rowvec ? p.rowvec + (long long)batch_idx * p.rowvec_ld : nullptr;
+                if (p.act == 2) {
+                    // GEGLU: accumulator columns come in groups of 32 = [16 value | 16 gate]; this thread holds value column
+                    // 8 b + cq (+1) of group g in block 4 g + b and its gate 16 columns later in block 4 g + b + 2
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (n0 + j < p.N) v[j] = fmaf(v[j], st.x, -st.y * __ldg(p.ln_colsum + n0 + j));
+                    for (int g = 0; g < BN / 32; ++g) {
+                        if (nt * BN + g * 32 >= p.N) break;
+#pragma unroll
+                        for (int b = 0; b < 2; ++b) {
+                            const int nv = nt * BN + g * 32 + b * 8 + cq;
+                            float xv0 = acc[4 * (4 * g + b) + 2 * h], xv1 = acc[4 * (4 * g + b) + 2 * h + 1];
+                            float gv0 = acc[4 * (4 * g + b + 2) + 2 * h], gv1 = acc[4 * (4 * g + b + 2) + 2 * h + 1];
+                            if (p.bias) {
+                                xv0 += __ldg(p.bias + nv); xv1 += __ldg(p.bias + nv + 1);
+                                gv0 += __ldg(p.bias + nv + 16); gv1 += __ldg(p.bias + nv + 17);
+                            }
+                            if (rv) {
+                                xv0 += __ldg(rv + nv); xv1 += __ldg(rv + nv + 1);
+                                gv0 += __ldg(rv + nv + 16); gv1 += __ldg(rv + nv + 17);
+                            }
+                            float o0 = bf16_round(bf16_round(xv0) * bf16_round(gelu_erf_f(bf16_round(gv0))));
+                            float o1 = bf16_round(bf16_round(xv1) * bf16_round(gelu_erf_f(bf16_round(gv1))));
+                            const int oc = (nt * BN) / 2 + g * 16 + b * 8 + cq;
+                            if (p.residual) {
+                                const float2 r = load_res_pair(p, grow, oc, true);
+                                o0 += r.x; o1 += r.y;
+                            }
+                            store_pair(p, grow, oc, o0, o1, true);
+                        }
                     }
-                    if (p.bias) {
+                } else {
+                    float ln_rs = 1.f, ln_nm = 0.f;
+                    if (p.ln_stats) { const float2 st = __ldg(p.ln_stats + grow); ln_rs = st.x; ln_nm = st.y; }
 #pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (n0 + j < p.N) v[j] += __ldg(p.bias + n0 + j);
-                    }
-                    if (p.rowvec) {
-                        const float* rv = p.rowvec + (long long)batch_idx * p.rowvec_ld + n0;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (n0 + j < p.N) v[j] += __ldg(rv + j);
-                    }
-                    if (p.act == 2) {
-                        // GEGLU: accumulator columns come in groups of 32 = [16 value | 16 gate]
-                        const int o0 = (n0 >> 5) * 16;
-                        float o[16];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            o[j] = bf16_round(bf16_round(v[j]) * bf16_round(gelu_erf_f(bf16_round(v[16 + j]))));
-                        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.ldc + o0;
+                    for (int j = 0; j < BN / 8; ++j) {
+                        const int n = nt * BN + 8 * j + cq;
+                        if (n >= p.N) break;
+                        const bool n1ok = n + 1 < p.N;
+                        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                        if (p.ln_stats) {
+                            v0 = fmaf(v0, ln_rs, -ln_nm * __ldg(p.ln_colsum + n));
+                            if (n1ok) v1 = fmaf(v1, ln_rs, -ln_nm * __ldg(p.ln_colsum + n + 1));
+                        }
+                        if (p.bias) { v0 += __ldg(p.bias + n); if (n1ok) v1 += __ldg(p.bias + n + 1); }
+                        if (rv) { v0 += __ldg(rv + n); if (n1ok) v1 += __ldg(rv + n + 1); }
+                        if (p.act == 1) { v0 = silu_f(bf16_round(v0)); v1 = silu_f(bf16_round(v1)); }
                         if (p.residual) {
-                            const __nv_bfloat16* rs = p.residual + grow * p.ldr + o0;
-#pragma unroll
-                            for (int j = 0; j < 16; ++j)
-                                if (o0 + j < p.n_out) o[j] += __bfloat162float(rs[j]);
+                            const float2 r = load_res_pair(p, grow, n, n1ok);
+                            if (p.out_f32) { v0 += r.x; v1 += r.y; }
+                            else { v0 = bf16_round(v0) + r.x; v1 = bf16_round(v1) + r.y; }
                         }
-                        if (o0 + 16 <= p.n_out && ((p.ldc & 7) == 0)) {
-                            uint4 q0, q1;
-                            q0.x = pack_bf16x2(o[0], o[1]);   q0.y = pack_bf16x2(o[2], o[3]);
-                            q0.z = pack_bf16x2(o[4], o[5]);   q0.w = pack_bf16x2(o[6], o[7]);
-                            q1.x = pack_bf16x2(o[8], o[9]);   q1.y = pack_bf16x2(o[10], o[11]);
-                            q1.z = pack_bf16x2(o[12], o[13]); q1.w = pack_bf16x2(o[14], o[15]);
-                            reinterpret_cast<uint4*>(dst)[0] = q0;
-                            reinterpret_cast<uint4*>(dst)[1] = q1;
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j)
-                                if (o0 + j < p.n_out) dst[j] = __float2bfloat16_rn(o[j]);
-                        }
-                    } else {
-                        if (p.act == 1) {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] = silu_f(bf16_round(v[j]));
-                        }
-                        if (p.out_f32) {
-                            float* dst = reinterpret_cast<float*>(p.out) + grow * p.ldc + n0;
-                            if (p.residual) {
-                                const __nv_bfloat16* rs = p.residual + grow * p.ldr + n0;
-#pragma unroll
-                                for (int j = 0; j < 32; ++j)
-                                    if (n0 + j < p.N) v[j] += __bfloat162float(rs[j]);
-                            }
-#pragma unroll
-                            for (int j = 0; j < 32; ++j)
-                                if (n0 + j < p.N) dst[j] = v[j];
-                        } else {
-                            __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.ldc + n0;
-                            const bool vec_ok = (n0 + 32 <= p.N) && ((p.ldc & 7) == 0) &&
-                                                ((reinterpret_cast<uintptr_t>(p.out) & 15) == 0);
-                            if (p.residual) {
-                                const __nv_bfloat16* rs = p.residual + grow * p.ldr + n0;
-                                if (vec_ok && ((p.ldr & 7) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0)) {
-                                    const uint4* rq = reinterpret_cast<const uint4*>(rs);
-#pragma unroll
-                                    for (int q = 0; q < 4; ++q) {
-                                        const uint4 u = __ldg(rq + q);
-                                        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-                                        for (int t = 0; t < 4; ++t) {
-                                            const float2 f = unpack_bf16x2(w[t]);
-                                            v[q * 8 + t * 2] = bf16_round(v[q * 8 + t * 2]) + f.x;
-                                            v[q * 8 + t * 2 + 1] = bf16_round(v[q * 8 + t * 2 + 1]) + f.y;
-                                        }
-                                    }
-                                } else {
-#pragma unroll
-                                    for (int j = 0; j < 32; ++j)
-                                        if (n0 + j < p.N) v[j] = bf16_round(v[j]) + __bfloat162float(rs[j]);
-                                }
-                            }
-                            if (vec_ok) {
-                                uint4* dq = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-                                for (int q = 0; q < 4; ++q) {
-                                    uint4 u;
-                                    u.x = pack_bf16x2(v[q * 8 + 0], v[q * 8 + 1]);
-                                    u.y = pack_bf16x2(v[q * 8 + 2], v[q * 8 + 3]);
-                                    u.z = pack_bf16x2(v[q * 8 + 4], v[q * 8 + 5]);
-                                    u.w = pack_bf16x2(v[q * 8 + 6], v[q * 8 + 7]);
-                                    dq[q] = u;
-                                }
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j)
-                                    if (n0 + j < p.N) dst[j] = __float2bfloat16_rn(v[j]);
-                            }
-                        }
+                        store_pair(p, grow, n, v0, v1, n1ok);
                     }
                 }
-            };
-            // software pipeline over this warp's chunks: the tcgen05.ld of the next chunk overlaps the stores of this one
-            constexpr int NCH = BN / 32;
-            uint32_t ra[32], rb[32];
-            int c = half;
-            if (c < NCH && nt * BN + c * 32 < p.N) tmem_ld_32x32(t_row + c * 32, ra);
-#pragma unroll 1
-            for (; c < NCH; c += 4) {
-                if (nt * BN + c * 32 >= p.N) break;                       // warp-uniform
-                tmem_ld_wait();
-                const int c2 = c + 2;
-                const bool has2 = c2 < NCH && nt * BN + c2 * 32 < p.N;
-                if (has2) tmem_ld_32x32(t_row + c2 * 32, rb);
-                process(ra, c * 32);
-                if (!has2) break;
-                tmem_ld_wait();
-                const int c4 = c + 4;
-                if (c4 < NCH && nt * BN + c4 * 32 < p.N) tmem_ld_32x32(t_row + c4 * 32, ra);
-                process(rb, c2 * 32);
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { if (CTAS == 2 && cta_rank != 0) mbar_arrive_cluster(&tmem_empty[acc], 0); else mbar_arrive(&tmem_empty[acc]); }
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (CTAS == 2) cluster_sync_all();     // CTA 0's MMAs read the peer's shared memory: nobody leaves before both are done
-    if (warp == 1) {
-        tc_fence_after();
-        if (CTAS == 2) tmem_dealloc_2sm(tmem_base, S::TMEM_COLS); else tmem_dealloc(tmem_base, S::TMEM_COLS);
     }
 }
 
@@ -681,90 +361,39 @@ int device_sm_count() {
     const int d = current_device_slot();
     if (sms[d] == 0) {
         cudaDeviceGetAttribute(&sms[d], cudaDevAttrMultiProcessorCount, d);
-        if (sms[d] <= 0) sms[d] = 148;
+        if (sms[d] <= 0) sms[d] = 132;
     }
     return sms[d];
 }
 
 extern int g_force_bn;
-extern long long g_desc_override;
-extern long long g_idesc_override;
 
-extern int g_gemm_pair;
-
-// CTA-pair (tcgen05 cta_group::2) mode: a 2-CTA cluster computes a 256 x BN tile, each CTA loading only half of the W tile.
-// Halves the shared-memory fill traffic per flop for W; used for the widest tile when there are enough row tiles.
-static int gemm_pair_mode() {
-    if (g_gemm_pair < 0) {
-        const char* e = getenv("SUPIR_B200_GEMM_PAIR");
-        g_gemm_pair = e ? atoi(e) : 1;
-    }
-    return g_gemm_pair;
-}
-// mode 0: never; 1: where it measured faster (profiles/r01_selftest_pair.log) — not the short-K GEGLU GEMMs, whose
-// epilogue-bound pipeline loses more to the pair's coupled accumulator hand-off than the mainloop gains; 2: always
-static int pick_ctas(const GemmKernelParams& p, int bn) {
-    const int mode = gemm_pair_mode();
-    if (mode == 0 || bn < 128 || p.num_m_tiles < 2) return 1;
-    if (mode == 1) {
-        if (p.act == 2 && p.num_kb < 16) return 1;
-        // the narrower tiles only gain from pairing when the mainloop is long (K >= 4096) and hurt below that
-        if (bn < 256 && (p.conv || p.num_kb < 64)) return 1;
-    }
-    return 2;
-}
-
-template <int BN, int CTAS>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmR,
-                       GemmKernelParams p, cudaStream_t st) {
-    using S = GemmSmem<BN, CTAS>;
+template <int BN>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKernelParams p, cudaStream_t st) {
+    using S = GemmSmem<BN>;
     static bool attr_set[64] = {};
     const int dslot = current_device_slot();
     if (!attr_set[dslot]) {
-        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(gemm_tcgen05_kernel<BN, CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
         attr_set[dslot] = true;
     }
     p.num_n_tiles = (p.N + BN - 1) / BN;
     p.nimg = p.conv ? (int)(p.M / ((long long)p.H * p.W)) : 0;
     {
-        uint64_t dt = g_desc_override >= 0 ? (uint64_t)g_desc_override
-                                           : (((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61));
-        p.desc_hi = (uint32_t)(dt >> 32);
-        p.desc_lbo = (uint32_t)(dt & 0xFFFFFFFFu);
-        p.idesc = g_idesc_override >= 0 ? (uint32_t)g_idesc_override : umma_idesc_bf16(BM * CTAS, BN);
-    }
-    {
-        // tile order that minimises HBM traffic under a simple L2 model: the CTAs running together (one round) either share
-        // a W tile (m-fastest; A is re-streamed once per n-tile unless it fits L2) or share an A tile (n-fastest; W is
-        // re-streamed once per round of m-tiles unless it fits L2)
-        const double l2 = 64e6;
+        // tile order that minimises HBM traffic under a simple L2 model (50 MB of L2 on H100): the CTAs running together
+        // (one round) either share a W tile (m-fastest; A is re-streamed once per n-tile unless it fits L2) or share an A tile
+        // (n-fastest; W is re-streamed once per round of m-tiles unless it fits L2)
+        const double l2 = 50e6;
         const double a_bytes = 2.0 * p.M * (p.conv ? p.Cin : p.K), w_bytes = 2.0 * p.N * p.K;
         const double rounds_m = (double)p.num_m_tiles * p.num_n_tiles / device_sm_count();
         const double t_mfast = w_bytes + (a_bytes <= l2 ? a_bytes : a_bytes * p.num_n_tiles);
         const double t_nfast = a_bytes + (w_bytes <= l2 ? w_bytes : w_bytes * (rounds_m < 1 ? 1 : rounds_m));
         p.m_fastest = t_mfast < t_nfast ? 1 : 0;
     }
-    p.num_m_tiles = (p.num_m_tiles + CTAS - 1) / CTAS;     // from here on: tiles of 128 * CTAS rows
     const int tiles = p.num_m_tiles * p.num_n_tiles;
-    const int slots = device_sm_count() / CTAS;
-    const int grid = CTAS * (tiles < slots ? tiles : slots);
-    if (CTAS == 1) {
-        gemm_tcgen05_kernel<BN, CTAS><<<grid, GEMM_THREADS, S::TOTAL, st>>>(tmA, tmB, tmC, tmR, p);
-    } else {
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(grid);
-        cfg.blockDim = dim3(GEMM_THREADS);
-        cfg.dynamicSmemBytes = S::TOTAL;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = CTAS;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        SUPIR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_tcgen05_kernel<BN, CTAS>, tmA, tmB, tmC, tmR, p));
-    }
+    const int slots = device_sm_count();
+    const int grid = tiles < slots ? tiles : slots;
+    gemm_wgmma_kernel<BN><<<grid, GEMM_THREADS, S::TOTAL, st>>>(tmA, tmB, p);
     count_launch();
     SUPIR_CHECK_CUDA(cudaGetLastError());
     return SUPIR_OK;
@@ -784,9 +413,10 @@ static int pick_bn(const GemmKernelParams& p, int force_bn) {
         if (bn > 64 && N <= bn / 2) continue;
         const long long tiles = (long long)m_tiles * ((N + bn - 1) / bn);
         const long long rounds = (tiles + sms - 1) / sms;
-        // MMA time of a tile ~ bn * num_kb (narrow tiles are shared-memory bound: 128-wide costs ~1.15x per column, 64-wide ~1.5x);
-        // plus a per-tile overhead (pipeline fill + epilogue not hidden on the last tile) of ~6 k-blocks of a 256-wide tile
-        const double per_col = bn == 256 ? (pick_ctas(p, 256) == 2 ? 0.9 : 1.0) : (bn == 160 ? 1.2 : (bn == 128 ? 1.42 : 2.0));   // measured (profiles/r01_*perf2*)
+        // MMA time of a tile ~ bn * num_kb, with a per-column penalty for narrow tiles (each k-block re-reads the whole A
+        // tile from shared memory for fewer columns); plus a per-tile overhead (pipeline fill + epilogue, which does not
+        // overlap the next tile's MMAs) of ~6 k-blocks of a 256-wide tile. Relative estimates, not measurements.
+        const double per_col = bn == 256 ? 1.0 : (bn == 160 ? 1.1 : (bn == 128 ? 1.2 : 1.6));
         const double tile_cost = bn * per_col * num_kb + 256.0 * 6.0;
         const double cost = rounds * tile_cost;
         if (cost < best_cost - 1e-9) { best_cost = cost; best = bn; }
@@ -795,86 +425,13 @@ static int pick_bn(const GemmKernelParams& p, int force_bn) {
 }
 
 int g_force_bn = 0;
-int g_gemm_pair = -1;             // CTA-pair (cta_group::2) kernel for the 256-wide tile: 0 never, 1 heuristic, 2 always; -1 = env/default
-long long g_desc_override = -1;   // debug: full 64-bit descriptor template (address bits zero), -1 = default
-long long g_idesc_override = -1;  // debug: instruction descriptor, -1 = default
-
-int g_force_direct_epilogue = 0;   // debug: 1 disables the staged (smem + TMA store) epilogue
-int g_warp_epilogue = -1;          // staged epilogue: 0 = one TMA op per 128-row chunk (named barriers), 1 = per-warp 32-row TMA ops; -1 = env / automatic
-static int g_warp_epilogue_env = -2;
-static int gemm_epilogue_mode() {
-    if (g_warp_epilogue >= 0) return g_warp_epilogue;
-    if (g_warp_epilogue_env == -2) {
-        const char* e = getenv("SUPIR_B200_GEMM_WARP_EPILOGUE");
-        g_warp_epilogue_env = e ? (atoi(e) != 0) : -1;
-    }
-    return g_warp_epilogue_env;
-}
-
-// staged epilogue applies to bf16 outputs with 16-byte aligned rows; it needs the per-image vector to be uniform per tile
-static bool can_stage(const GemmKernelParams& p) {
-    if (g_force_direct_epilogue || p.out_f32) return false;
-    if (p.conv && (p.out_sy != 1 || p.out_sx != 1)) return false;     // interleaved (sub-pixel) outputs: per-row addresses
-    if ((p.ldc & 7) || (reinterpret_cast<uintptr_t>(p.out) & 15)) return false;
-    if (p.n_out < (p.act == 2 ? 16 : 32)) return false;
-    if (p.rowvec && !p.conv) return false;
-    if (p.residual && (p.act == 2 || (p.ldr & 7) || (reinterpret_cast<uintptr_t>(p.residual) & 15))) return false;
-    return true;
-}
-
-// output / residual tensor maps of the staged epilogue: 32-column (GEGLU: 16-column) chunks of the tile's 128 rows
-static int make_epi_maps(const GemmKernelParams& p, CUtensorMap* tmC, CUtensorMap* tmR) {
-    const uint32_t cols = p.act == 2 ? 16 : 32;
-    const int sw = p.act == 2 ? 32 : 64;
-    int rc;
-    if (p.conv) {
-        const uint64_t dims[4] = {(uint64_t)p.n_out, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)(p.M / ((long long)p.H * p.W))};
-        const uint32_t bw = p.TW < 32 ? p.TW : 32;                      // warp_epi: one warp's 32 pixels of the TH x TW patch
-        const uint32_t box_full[4] = {cols, (uint32_t)p.TW, (uint32_t)p.TH, 1}, box_warp[4] = {cols, bw, 32 / bw, 1};
-        const uint32_t* box = p.warp_epi ? box_warp : box_full;
-        const uint64_t sc[3] = {(uint64_t)p.ldc, (uint64_t)p.ldc * p.W, (uint64_t)p.ldc * p.W * p.H};
-        if ((rc = make_tmap_bf16_sw(tmC, p.out, 4, dims, sc, box, sw))) return rc;
-        if (p.residual) {
-            const uint64_t sr[3] = {(uint64_t)p.ldr, (uint64_t)p.ldr * p.W, (uint64_t)p.ldr * p.W * p.H};
-            if ((rc = make_tmap_bf16_sw(tmR, p.residual, 4, dims, sr, box, sw))) return rc;
-        }
-    } else {
-        const uint64_t dims[2] = {(uint64_t)p.n_out, (uint64_t)p.M};
-        const uint32_t box[2] = {cols, (uint32_t)(p.warp_epi ? 32 : BM)};
-        const uint64_t sc[1] = {(uint64_t)p.ldc};
-        if ((rc = make_tmap_bf16_sw(tmC, p.out, 2, dims, sc, box, sw))) return rc;
-        if (p.residual) {
-            const uint64_t sr[1] = {(uint64_t)p.ldr};
-            if ((rc = make_tmap_bf16_sw(tmR, p.residual, 2, dims, sr, box, sw))) return rc;
-        }
-    }
-    return SUPIR_OK;
-}
 
 static int run_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKernelParams& p, cudaStream_t st) {
-    CUtensorMap tmC = tmA, tmR = tmA;   // placeholders when the direct epilogue is used
-    p.staged = can_stage(p) ? 1 : 0;
-    p.has_res = (p.staged && p.residual) ? 1 : 0;
-    // per-warp TMA epilogue: +6..21 % on the bias / residual epilogues of the step's GEMMs, -2..5 % on GEGLU (whose chunks are
-    // 16 columns wide: 1 KB per warp and store) — profiles/r02_selftest_epiperf.log; convolutions keep the group mode (their
-    // per-warp boxes are 2-4 image-row fragments; the step's convs measured ~10 % slower with them). -1 = that rule; 0 / 1
-    // force a mode.
-    const int em = gemm_epilogue_mode();
-    p.warp_epi = (p.staged && (em < 0 ? (p.act != 2 && !p.conv) : em != 0)) ? 1 : 0;
-    if (p.staged) {
-        const int rc = make_epi_maps(p, &tmC, &tmR);
-        if (rc) return rc;
-    }
     const int bn = pick_bn(p, g_force_bn);
-    if (pick_ctas(p, bn) == 2) {
-        if (bn == 256) return launch_gemm<256, 2>(tmA, tmB, tmC, tmR, p, st);
-        if (bn == 160) return launch_gemm<160, 2>(tmA, tmB, tmC, tmR, p, st);
-        return launch_gemm<128, 2>(tmA, tmB, tmC, tmR, p, st);
-    }
-    if (bn == 256) return launch_gemm<256, 1>(tmA, tmB, tmC, tmR, p, st);
-    if (bn == 160) return launch_gemm<160, 1>(tmA, tmB, tmC, tmR, p, st);
-    if (bn == 128) return launch_gemm<128, 1>(tmA, tmB, tmC, tmR, p, st);
-    return launch_gemm<64, 1>(tmA, tmB, tmC, tmR, p, st);
+    if (bn == 256) return launch_gemm<256>(tmA, tmB, p, st);
+    if (bn == 160) return launch_gemm<160>(tmA, tmB, p, st);
+    if (bn == 128) return launch_gemm<128>(tmA, tmB, p, st);
+    return launch_gemm<64>(tmA, tmB, p, st);
 }
 
 static int fill_epilogue(GemmKernelParams& p, const supir_epilogue* ep, int N) {
@@ -910,27 +467,6 @@ static int fill_epilogue(GemmKernelParams& p, const supir_epilogue* ep, int N) {
 
 using namespace supir;
 
-extern "C" int supir_debug_set_umma_descriptors(long long smem_desc_template, long long idesc) {
-    g_desc_override = smem_desc_template;
-    g_idesc_override = idesc;
-    return SUPIR_OK;
-}
-
-extern "C" int supir_debug_force_direct_epilogue(int on) {
-    g_force_direct_epilogue = on;
-    return SUPIR_OK;
-}
-
-extern "C" int supir_set_gemm_epilogue_mode(int per_warp) {
-    g_warp_epilogue = per_warp < 0 ? -1 : (per_warp != 0);
-    return SUPIR_OK;
-}
-
-extern "C" int supir_set_gemm_pair_mode(int on) {
-    g_gemm_pair = on < 0 ? 0 : (on > 2 ? 2 : on);
-    return SUPIR_OK;
-}
-
 extern "C" int supir_set_gemm_tile_n(int bn) {
     g_force_bn = bn;
     return SUPIR_OK;
@@ -963,7 +499,7 @@ extern "C" int supir_gemm_bf16(const void* A, long long lda, const void* W, long
     {
         const uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
         const uint64_t str[1] = {(uint64_t)ldw};
-        const uint32_t box[2] = {BK, (uint32_t)(bn / pick_ctas(p, bn))};
+        const uint32_t box[2] = {BK, (uint32_t)bn};
         rc = make_tmap_bf16(&tmB, W, 2, dims, str, box);
         if (rc) return rc;
     }
@@ -1024,7 +560,7 @@ static int conv_geom_impl(const char* who, const void* x, long long ldx, const v
     {
         const uint64_t dims[2] = {(uint64_t)(ntaps * Cin), (uint64_t)Cout};
         const uint64_t str[1] = {(uint64_t)(ntaps * Cin)};
-        const uint32_t box[2] = {BK, (uint32_t)(bn / pick_ctas(p, bn))};
+        const uint32_t box[2] = {BK, (uint32_t)bn};
         rc = make_tmap_bf16(&tmB, Wp, 2, dims, str, box);
         if (rc) return rc;
     }

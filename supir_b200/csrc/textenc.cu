@@ -1,6 +1,6 @@
 // supir_b200 — kernels of the text conditioner (SURVEY.md §8(f)2): the CLIP-L and OpenCLIP bigG text towers run ONCE per
 // image on 77 tokens (sgm/modules/encoders/modules.py:484-507, 553-609), so nothing here is throughput-critical: the
-// projections go through the tcgen05 GEMM of gemm.cu, and the pieces that GEMM does not cover are these small CUDA-core
+// projections go through the wgmma GEMM of gemm.cu, and the pieces that GEMM does not cover are these small CUDA-core
 // kernels — token / position embedding gather, LayerNorm on the fp32 residual stream (the reference keeps that stream in fp32:
 // autocast only lowers the matmuls), causal attention over <= 128 tokens, and the MLP activations (quick-GELU for CLIP-L,
 // exact GELU for bigG).
@@ -11,7 +11,7 @@ namespace supir {
 
 static inline unsigned te_blocks_for(long long n, int threads) {
     long long b = (n + threads - 1) / threads;
-    const long long cap = 148LL * 16;
+    const long long cap = device_sm_count() * 16LL;   // grid-stride loops: 16 blocks per SM
     if (b > cap) b = cap;
     if (b < 1) b = 1;
     return (unsigned)b;
@@ -193,7 +193,7 @@ extern "C" int supir_layernorm_f32(const float* x, long long ldx, void* y_bf16, 
     SUPIR_REQUIRE(ldx >= C && (!y_bf16 || ldyb >= C) && (!y_f32 || ldyf >= C), "supir_layernorm_f32: leading dims smaller than C");
     const int warps = 8;
     long long blocks = (rows + warps - 1) / warps;
-    if (blocks > 148LL * 8) blocks = 148LL * 8;
+    if (blocks > device_sm_count() * 8LL) blocks = device_sm_count() * 8LL;
     layernorm_f32_kernel<<<(unsigned)blocks, warps * 32, 0, ST(stream)>>>(x, ldx, BF(y_bf16), ldyb, y_f32, ldyf, rows, C, gamma, beta, eps);
     DONE();
 }

@@ -1,4 +1,4 @@
-"""SUPIRModel engine on the B200 backend (reference: SUPIR/models/SUPIR_model.py:12-179 on top of
+"""SUPIRModel engine on the H100 backend (reference: SUPIR/models/SUPIR_model.py:12-179 on top of
 sgm/models/diffusion.py:22-83).
 
 The reference keeps this layer as Python orchestration (stage-1 encode/decode, conditioning, sampler call, decode); it is

@@ -1,10 +1,10 @@
-"""GLVControl / LightGLVUNet for the B200 backend.
+"""GLVControl / LightGLVUNet for the H100 backend.
 
 Same constructor parameters and state_dict key names as the reference classes (SUPIR/modules/SUPIR_v0.py:155-666,
 sgm/modules/diffusionmodules/openaimodel.py:506-961, sgm/modules/attention.py:196-635) so the reference's YAML configs and
 checkpoints load unchanged — but the torch modules below only OWN parameters. Nothing here runs a torch op on the hot
 path: `pack()` converts the weights once into the kernel layouts (bf16, K-major, fused QKV / KV / GEGLU / gamma|beta
-matrices, fp32 biases) and `run()` issues hand-written sm_100a kernels through the C ABI (supir_b200/ops.py) on
+matrices, fp32 biases) and `run()` issues hand-written sm_90a kernels through the C ABI (supir_b200/ops.py) on
 channels-last bf16 activations. Options the SUPIR configs never use raise NotImplementedError.
 """
 import os

@@ -72,7 +72,7 @@ class Pool:
     def trim(self):
         """Drop the cached free buffers (they go back to torch's caching allocator); tensors still in use stay with their
         holders. For pools OUTSIDE a CUDA graph only (the tiled VAE: a 256-tile pass touches four resolutions whose scratch
-        sizes never recur, and keeping all of them cached would not fit 180 GB)."""
+        sizes never recur, and keeping all of them cached would not fit 80 GB)."""
         self.free.clear()
         self.all = []
 

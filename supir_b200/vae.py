@@ -1,4 +1,4 @@
-"""SDXL VAE (encoder / decoder / AutoencoderKL wrapper) and the tiled VAE for the B200 backend.
+"""SDXL VAE (encoder / decoder / AutoencoderKL wrapper) and the tiled VAE for the H100 backend.
 
 Reference: sgm/modules/diffusionmodules/model.py:49-148,158-262,482-743 (Encoder/Decoder/ResnetBlock/AttnBlock),
 sgm/models/autoencoder.py:282-321 (AutoencoderKL[InferenceWrapper]), sgm/modules/distributions/distributions.py:24-41,
@@ -22,10 +22,10 @@ from .nets import Act, _bf, _bias_bf16_values, _f32, pack_conv3x3
 from .ops import BF16
 
 
-# cached scratch above this is handed back to torch's allocator between resolutions (many-tile images: an 8192^2 pass would
-# otherwise keep ~170 GB of four resolutions' buffers cached). High enough that the 4096^2 workload (26 GB) never trims:
-# re-acquiring trimmed buffers costs cudaMalloc time (a ~1 s spike was measured in one bench run with a 24 GB threshold).
-POOL_TRIM_BYTES = 64 << 30
+# cached scratch above this is handed back to torch's caching allocator between resolutions and after a pass. The three VAE
+# networks of a restore (denoise encoder, decoder, encoder) each own a pool, and on an 80 GB H100 they cannot each keep the
+# ~26 GB a 4096^2 pass uses: above 8 GB the buffers go back to torch's allocator, where the next network's pass reuses them.
+POOL_TRIM_BYTES = 8 << 30
 
 
 def Normalize(in_channels, num_groups=32):

@@ -1,9 +1,9 @@
 """GPU parity of the tensor-core kernels AT THE SHAPES bench.py TIMES (the batch-98 denoiser call of BASELINE configs[2]:
 49 windows x CFG pair, 128x128 latent windows), through the C ABI, against plain PyTorch fp32 maths on the same
-bf16-rounded operands. The shape list is the GEMM-class launch list of that call (profiles/r01_breakdown_batch98.txt,
-SURVEY.md §8a rows a8/a9): every epilogue the networks use, every N tile the dispatcher can pick, CTA-pair mode on and off,
-the staged and the direct epilogue. Attention covers the two self-attention shapes of the step, ragged key counts and
-adversarial logits that force the lazy O rescale (attention.cu) in every key block.
+bf16-rounded operands. The shape list is the GEMM-class launch list of that call (SURVEY.md §8a rows a8/a9): every
+epilogue the networks use, every N tile the dispatcher can pick, bf16 and fp32 outputs.
+Attention covers the two self-attention shapes of the step, ragged key counts and adversarial logits that move the
+online-softmax row maximum (and so rescale O) in every key block.
 
 Tolerance (bf16 storage, fp32 accumulation, vs fp32): |err| <= 2e-2 + 2e-2 |ref| per element for GEMM / conv outputs of
 unit scale; attention: |err| <= 1.5e-2 |ref| + 4e-3 max|ref| and relative Frobenius error <= 5e-3.
@@ -61,7 +61,7 @@ def _check(got, ref, what, atol=2e-2, rtol=2e-2):
     assert bool(torch.isfinite(got.float()).all()), what
 
 
-# (M, N, K, act, bias, residual): the GEMM-class launches that carry the step (count x time in profiles/r01_breakdown_batch98.txt)
+# (M, N, K, act, bias, residual): the GEMM-class launches that carry the step
 GEMM_SHAPES = [
     (M1, 10240, 1280, 2, True, False),    # FeedForward GEGLU proj, 1280-ch level (90 per call)
     (M1, 1280, 5120, 0, True, True),      # FeedForward out + residual
@@ -88,29 +88,17 @@ def test_gemm_bench_shapes_all_tiles_and_pair_modes(shape):
     ref = _ref_gemm(a, w, bias, res, act)
     lib = native.load()
     try:
-        for pair, epi in ((0, 0), (2, 0), (2, 1), (0, 1)):
-            for bn in (0, 64, 128, 160, 256):
-                lib.supir_set_gemm_pair_mode(pair)
-                lib.supir_set_gemm_epilogue_mode(epi)
-                lib.supir_set_gemm_tile_n(bn)
-                out = torch.full((M, n_out), float("nan"), dtype=BF, device="cuda")
-                ops.gemm(a, w, out, bias=bias, residual=res, act=act)
-                _check(out, ref, f"gemm {shape} tile_n={bn} pair={pair} warp_epilogue={epi}")
-        # direct-store epilogue (the fallback for fp32 outputs / unaligned shapes) at the same shape
-        lib.supir_set_gemm_pair_mode(1)
+        for bn in (0, 64, 128, 160, 256):
+            lib.supir_set_gemm_tile_n(bn)
+            out = torch.full((M, n_out), float("nan"), dtype=BF, device="cuda")
+            ops.gemm(a, w, out, bias=bias, residual=res, act=act)
+            _check(out, ref, f"gemm {shape} tile_n={bn}")
         lib.supir_set_gemm_tile_n(0)
-        lib.supir_debug_force_direct_epilogue(1)
-        out = torch.full((M, n_out), float("nan"), dtype=BF, device="cuda")
-        ops.gemm(a, w, out, bias=bias, residual=res, act=act)
-        _check(out, ref, f"gemm {shape} direct epilogue")
         if act != 2:
             out32 = torch.full((M, n_out), float("nan"), dtype=torch.float32, device="cuda")
             ops.gemm(a, w, out32, bias=bias, residual=res, act=act)
             _check(out32, ref, f"gemm {shape} fp32 out")
     finally:
-        lib.supir_debug_force_direct_epilogue(0)
-        lib.supir_set_gemm_epilogue_mode(-1)
-        lib.supir_set_gemm_pair_mode(1)
         lib.supir_set_gemm_tile_n(0)
 
 
@@ -155,16 +143,12 @@ def test_conv3x3_bench_shapes(shape):
         ref[b0 * H * W:(b0 + nb) * H * W] = y
     lib = native.load()
     try:
-        for pair, bn, epi in ((1, 0, 0), (0, 256, 0), (2, 256, 0), (0, 128, 0), (0, 160, 0), (0, 64, 0), (1, 0, 1), (2, 256, 1), (0, 128, 1)):
-            lib.supir_set_gemm_pair_mode(pair)
-            lib.supir_set_gemm_epilogue_mode(epi)
+        for bn in (0, 256, 160, 128, 64):
             lib.supir_set_gemm_tile_n(bn)
             out = torch.full((B * H * W, Cout), float("nan"), dtype=BF, device="cuda")
             ops.conv3x3(x, B, H, W, wp, out, bias=bias, rowvec=rv, residual=res, act=act)
-            _check(out, ref, f"conv {shape} tile_n={bn} pair={pair} warp_epilogue={epi}")
+            _check(out, ref, f"conv {shape} tile_n={bn}")
     finally:
-        lib.supir_set_gemm_epilogue_mode(-1)
-        lib.supir_set_gemm_pair_mode(1)
         lib.supir_set_gemm_tile_n(0)
 
 

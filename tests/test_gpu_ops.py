@@ -122,7 +122,7 @@ def test_small_convs_and_conv1x1():
 
 
 def test_entry_exit_convs_on_tensor_cores_match_cuda_core_kernels():
-    """Large images route the Cin<=8 / Cout<=8 convs through im2col + tcgen05 GEMM / the padded implicit-GEMM conv
+    """Large images route the Cin<=8 / Cout<=8 convs through im2col + wgmma GEMM / the padded implicit-GEMM conv
     (ops.conv3x3_small_cin / _small_cout with packed weights): same values as the CUDA-core kernels and as torch."""
     ops = _ops()
     pool = ops.Pool()
@@ -339,16 +339,9 @@ def test_gemm_with_folded_layernorm(M, C, N, with_res):
     rstd = (xf.var(1, unbiased=False) + 1e-5).rsqrt()
     close(stats[:, 0].cpu(), rstd, 1e-4, 1e-4)
     close(stats[:, 1].cpu(), xf.mean(1) * rstd, 1e-4, 1e-4)
-    from supir_b200 import _native
-    lib = _native.load()
-    try:
-        for direct in (0, 1):
-            lib.supir_debug_force_direct_epilogue(direct)
-            out = torch.empty(M, N, dtype=BF, device="cuda")
-            ops.gemm(x.cuda(), wg, out, bias=b2, residual=None if res is None else res.cuda(), ln=(stats, c1))
-            close(out.float().cpu(), ref, 4e-2, 3e-2)
-    finally:
-        lib.supir_debug_force_direct_epilogue(0)
+    out = torch.empty(M, N, dtype=BF, device="cuda")
+    ops.gemm(x.cuda(), wg, out, bias=b2, residual=None if res is None else res.cuda(), ln=(stats, c1))
+    close(out.float().cpu(), ref, 4e-2, 3e-2)
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(2, 32, 32, 64, 96), (1, 37, 51, 128, 128), (3, 16, 24, 320, 320), (1, 150, 150, 64, 64)])

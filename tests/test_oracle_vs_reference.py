@@ -1,5 +1,5 @@
-"""Live re-derivation of the committed golden fixtures from the UNMODIFIED reference, whenever /root/reference is present
-(the build container; the GPU box has no reference and skips this file): the cheap generators of tests/golden/make_golden.py
+"""Live re-derivation of the committed golden fixtures from the UNMODIFIED reference, whenever its checkout is present
+(SUPIR_REFERENCE_ROOT; elsewhere this file skips): the cheap generators of tests/golden/make_golden.py
 are re-run into a scratch directory and must reproduce the committed files bit for bit. Together with
 tests/test_oracle_vs_golden.py (oracle == fixtures) this pins oracle == reference without trusting a stale fixture."""
 import importlib
@@ -12,7 +12,7 @@ import pytest
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
 import ref_stubs  # noqa: E402
 
-pytestmark = pytest.mark.skipif(not ref_stubs.reference_available(), reason="/root/reference not present (GPU box)")
+pytestmark = pytest.mark.skipif(not ref_stubs.reference_available(), reason="the reference checkout is not present")
 G = os.path.join(os.path.dirname(__file__), "golden")
 
 
@@ -30,6 +30,9 @@ def regen(tmp_path_factory):
         mg.gen_colorfix()
         mg.gen_conditioner()
         mg.gen_vae_fast()
+        mg.gen_util()
+        mg.gen_options()
+        mg.gen_prepared_conditioner()
     finally:
         mg.HERE = saved
     return str(out)
@@ -50,28 +53,14 @@ def test_bookkeeping_and_weights_regenerate_bit_identically(regen):
     _same_npz(os.path.join(regen, "gaussian_weights.npz"), os.path.join(G, "gaussian_weights.npz"))
 
 
-@pytest.mark.parametrize("name", ["zero_modules.npz", "glvcontrol_tiny.npz", "sampler_toy.npz", "colorfix.npz", "conditioner.npz", "vae_tiny_fast.npz"])
+@pytest.mark.parametrize("name", ["zero_modules.npz", "glvcontrol_tiny.npz", "sampler_toy.npz", "colorfix.npz", "conditioner.npz", "vae_tiny_fast.npz", "prepared_conditioner.npz"])
 def test_tensor_fixtures_regenerate_bit_identically(regen, name):
     _same_npz(os.path.join(regen, name), os.path.join(G, name))
 
 
-def test_pil2tensor_matches_reference_function():
-    """supir_b200.util.PIL2Tensor (host-side input preparation, restated) against the reference's own function
-    (SUPIR/util.py:60-84, executed from the read-only checkout) on random image sizes (24 of them) and every argument combination
-    test.py / gradio_demo use: same working size, same reported size, same pixels."""
-    import random
-    import torch
-    pytest.importorskip("PIL")
-    from PIL import Image
-    from supir_b200 import util
-    src = open("/root/reference/SUPIR/util.py").read()
-    ns = {"np": np, "torch": torch, "Image": Image}
-    exec(src[src.index("def PIL2Tensor"):src.index("def Tensor2PIL")], ns)
-    rng = random.Random(0)
-    for _ in range(24):
-        w, h = rng.randint(40, 900), rng.randint(40, 900)
-        img = Image.fromarray(np.random.RandomState(w * 1000 + h).randint(0, 255, (h, w, 3), dtype=np.uint8))
-        for up, ms, fr in [(1, 1024, None), (2, 1024, None), (4, 64, None), (1, 1024, 512), (3, 256, 512)]:
-            a = ns["PIL2Tensor"](img, upsacle=up, min_size=ms, fix_resize=fr)
-            b = util.PIL2Tensor(img, upsacle=up, min_size=ms, fix_resize=fr)
-            assert a[1:] == b[1:] and torch.equal(a[0], b[0]), (w, h, up, ms, fr)
+def test_util_fixture_and_options_regenerate_identically(regen):
+    with open(os.path.join(regen, "util_reference.json")) as f, open(os.path.join(G, "util_reference.json")) as g:
+        assert f.read() == g.read()
+    for name in sorted(os.listdir(os.path.join(G, "options"))):
+        with open(os.path.join(regen, "options", name), "rb") as f, open(os.path.join(G, "options", name), "rb") as g:
+            assert f.read() == g.read(), name

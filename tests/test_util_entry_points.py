@@ -1,6 +1,7 @@
 """supir_b200.util's model-construction entry points (SUPIR/util.py:11-57: create_SUPIR_model / load_QF_ckpt / load_state_dict /
 convert_dtype — what test.py and the gradio demos import) on synthetic checkpoints in both on-disk formats, driven by a YAML
 file with the layout of options/SUPIR_v0.yaml; and the small numpy helpers against the reference's own functions."""
+import json
 import os
 import sys
 
@@ -85,16 +86,33 @@ def get_keys(ckpt):
     return ckpt.get("state_dict", ckpt).keys()
 
 
-@pytest.mark.skipif(not ref_stubs.reference_available(), reason="/root/reference not present (GPU box)")
+def _reference_outputs():
+    with open(os.path.join(os.path.dirname(__file__), "golden", "util_reference.json")) as f:
+        return json.load(f)
+
+
 def test_numpy_helpers_match_the_reference_functions():
+    """HWC3 / Numpy2Tensor against what the reference's own functions (SUPIR/util.py) return on the same inputs, recorded
+    bit-exactly in tests/golden/util_reference.json by tests/golden/make_golden.py."""
+    from util_cases import array_digest, numpy_helper_inputs
     from supir_b200 import util
-    src = open(os.path.join(ref_stubs.REFERENCE_ROOT, "SUPIR", "util.py")).read()
-    ns = {"np": np, "torch": torch}
-    exec(src[src.index("def HWC3"):src.index("def upscale_image")], ns)
-    exec(src[src.index("def Numpy2Tensor"):src.index("def Tensor2Numpy")], ns)
-    rng = np.random.RandomState(0)
-    for shape in ((17, 23), (17, 23, 1), (17, 23, 3), (17, 23, 4)):
-        img = rng.randint(0, 256, shape).astype(np.uint8)
-        assert np.array_equal(util.HWC3(img), ns["HWC3"](img))
-    img = rng.randint(0, 256, (9, 11, 3)).astype(np.uint8)
-    assert torch.equal(util.Numpy2Tensor(img), ns["Numpy2Tensor"](img))
+    ref = _reference_outputs()
+    hwc3, img = numpy_helper_inputs()
+    assert [array_digest(util.HWC3(x)) for x in hwc3] == ref["hwc3"]
+    assert array_digest(util.Numpy2Tensor(img).numpy()) == ref["numpy2tensor"]
+
+
+def test_pil2tensor_matches_reference_function():
+    """supir_b200.util.PIL2Tensor (host-side input preparation, restated) against the reference's own function
+    (SUPIR/util.py:60-84) on random image sizes (24 of them) and every argument combination test.py / gradio_demo use: same
+    working size, same reported size, same pixels (the reference's outputs are recorded in tests/golden/util_reference.json)."""
+    pytest.importorskip("PIL")
+    from util_cases import PIL2TENSOR_CASES, array_digest, pil2tensor_images
+    from supir_b200 import util
+    ref = iter(_reference_outputs()["pil2tensor"])
+    for w, h, img in pil2tensor_images():
+        for up, ms, fr in PIL2TENSOR_CASES:
+            r = next(ref)
+            assert (r["w"], r["h"], r["upscale"], r["min_size"], r["fix_resize"]) == (w, h, up, ms, fr)
+            t, h0, w0 = util.PIL2Tensor(img, upsacle=up, min_size=ms, fix_resize=fr)
+            assert (h0, w0) == (r["h0"], r["w0"]) and array_digest(t.numpy()) == r["tensor"], (w, h, up, ms, fr)

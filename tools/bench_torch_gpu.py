@@ -1,4 +1,4 @@
-"""The reference's OWN GPU path timed on the B200 next to supir_b200 (SURVEY.md §8d last row, BASELINE.md §4 item 3: "the real
+"""The reference's OWN GPU path timed on the same GPU next to supir_b200 (SURVEY.md §8d last row, BASELINE.md §4 item 3: "the real
 competitor"): the oracle — a functional restatement of GLVControl + LightGLVUNet that calls exactly the torch ops the
 reference's modules call (F.linear / F.conv2d / F.group_norm / F.layer_norm / F.scaled_dot_product_attention) — run on
 `cuda` under `torch.autocast(bfloat16)` with bf16 weights (test.py --loading_half_params --diff_dtype bf16), eager mode like the

@@ -291,55 +291,6 @@ __global__ void fill_random_bf16(__nv_bfloat16* p, size_t n, float amp, uint32_t
     }
 }
 
-// step-realistic GEMM timing: random operands (power draw), bias (+ residual), 30 back-to-back launches
-static void perf_gemm_real(int M, int N, int K, int act, bool with_res, bool with_ln = false) {
-    const int n_out = act == 2 ? N / 2 : N;
-    __nv_bfloat16 *dA, *dW, *dOut, *dRes = nullptr;
-    float *dBias, *dStats = nullptr, *dC1 = nullptr;
-    CK(cudaMalloc(&dA, (size_t)M * K * 2));
-    CK(cudaMalloc(&dW, (size_t)N * K * 2));
-    CK(cudaMalloc(&dOut, (size_t)M * n_out * 2));
-    CK(cudaMalloc(&dBias, (size_t)N * 4));
-    CK(cudaMemset(dBias, 0, (size_t)N * 4));
-    fill_random_bf16<<<1024, 256>>>(dA, (size_t)M * K, 1.0f, 11u);
-    fill_random_bf16<<<1024, 256>>>(dW, (size_t)N * K, 0.05f, 12u);
-    supir_epilogue ep{};
-    ep.act = act;
-    ep.bias = dBias;
-    if (with_res) {
-        CK(cudaMalloc(&dRes, (size_t)M * n_out * 2));
-        fill_random_bf16<<<1024, 256>>>(dRes, (size_t)M * n_out, 1.0f, 13u);
-        ep.residual = dRes;
-        ep.ldr = n_out;
-    }
-    if (with_ln) {
-        CK(cudaMalloc(&dStats, (size_t)M * 8));
-        CK(cudaMalloc(&dC1, (size_t)N * 4));
-        CK(cudaMemset(dC1, 0, (size_t)N * 4));
-        supir_layernorm_stats(dA, K, M, K, 1e-5f, dStats, nullptr);
-        ep.ln_stats = dStats;
-        ep.ln_colsum = dC1;
-    }
-    for (int i = 0; i < 3; ++i) supir_gemm_bf16(dA, K, dW, K, dOut, n_out, M, N, K, &ep, nullptr);
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0); cudaEventCreate(&e1);
-    const int iters = 30;
-    cudaEventRecord(e0);
-    for (int i = 0; i < iters; ++i) supir_gemm_bf16(dA, K, dW, K, dOut, n_out, M, N, K, &ep, nullptr);
-    cudaEventRecord(e1);
-    CK(cudaEventSynchronize(e1));
-    float ms;
-    cudaEventElapsedTime(&ms, e0, e1);
-    ms /= iters;
-    printf("[PERF] gemm M=%d N=%d K=%d act=%d res=%d ln=%d : %.3f ms  %.1f TFLOP/s\n", M, N, K, act, (int)with_res, (int)with_ln, ms,
-           2.0 * M * N * K / ms / 1e9);
-    cudaFree(dA); cudaFree(dW); cudaFree(dOut); cudaFree(dBias);
-    if (dRes) cudaFree(dRes);
-    if (dStats) cudaFree(dStats);
-    if (dC1) cudaFree(dC1);
-    fflush(stdout);
-}
-
 static void perf_conv(int B, int H, int Wd, int Cin, int Cout, int bn) {
     __nv_bfloat16 *dX, *dW, *dOut;
     CK(cudaMalloc(&dX, (size_t)B * H * Wd * Cin * 2));
@@ -508,37 +459,12 @@ static void perf_gemm_variants(int M, int N, int K, int act) {
     cudaFree(dA); cudaFree(dW); cudaFree(dOut); cudaFree(dRes); cudaFree(cA); cudaFree(cW); cudaFree(dB);
 }
 
-// descriptor bring-up: try the default, then a few alternates, on a tiny identity GEMM
-static void bringup() {
-    printf("== bring-up: identity GEMM 128x64x64 with default descriptors\n");
-    supir_set_gemm_tile_n(64);
-    bool ok = test_gemm(128, 64, 64, 0, false, false, false, 0, true, true);
-    if (!ok) {
-        struct Var { const char* name; long long desc; } vars[] = {
-            {"version=1 sw128 sbo=1024 lbo=16", ((long long)(1024 >> 4) << 32) | (1LL << 46) | (2LL << 61) | (1LL << 16)},
-            {"version=0 sw128 sbo=1024 lbo=0", ((long long)(1024 >> 4) << 32) | (2LL << 61)},
-            {"version=0 sw128 sbo=1024 lbo=16", ((long long)(1024 >> 4) << 32) | (2LL << 61) | (1LL << 16)},
-            {"version=1 sw128(1<<62) sbo=1024", ((long long)(1024 >> 4) << 32) | (1LL << 46) | (1LL << 62)},
-        };
-        for (auto& v : vars) {
-            printf("-- variant: %s\n", v.name);
-            supir_debug_set_umma_descriptors(v.desc, -1);
-            if (test_gemm(128, 64, 64, 0, false, false, false, 0, true, true)) {
-                printf("   VARIANT WORKS: %s\n", v.name);
-                break;
-            }
-        }
-    }
-    supir_set_gemm_tile_n(0);
-}
-
 int main(int argc, char** argv) {
     std::string what = argc > 1 ? argv[1] : "all";
     int dev = 0;
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, dev));
     printf("device: %s sm_%d%d SMs=%d\n", prop.name, prop.major, prop.minor, prop.multiProcessorCount);
-    if (what == "bringup" || what == "all") bringup();
     if (what == "gemm" || what == "all") {
         for (int bn : {64, 128, 160, 256}) {
             supir_set_gemm_tile_n(bn);
@@ -553,7 +479,7 @@ int main(int argc, char** argv) {
         test_gemm(2048, 1280, 1280, 0, true, true, false, 20000);
         test_gemm(8192, 5120, 640, 2, true, false, false, 20000);
         test_gemm(2048, 2560, 1280, 2, true, true, false, 20000);
-        test_gemm(20000, 640, 640, 0, true, true, false, 20000);  // > 148 tiles: persistent loop + TMEM double buffer
+        test_gemm(20000, 640, 640, 0, true, true, false, 20000);  // > 132 tiles: the persistent tile loop wraps
     }
     if (what == "conv" || what == "all") {
         test_conv(1, 16, 16, 64, 64, 0, false, false);
@@ -563,57 +489,6 @@ int main(int argc, char** argv) {
         test_conv(2, 32, 32, 2560, 1280, 5000, false, true);
         test_conv(1, 150, 150, 128, 128, 20000, false, false);
         test_conv(2, 8, 8, 128, 256, 0, false, false);
-    }
-    if (what == "pair" || what == "all") {   // CTA-pair (cta_group::2) kernel: correctness, then speed against the 1-CTA kernel
-        supir_set_gemm_pair_mode(2);
-        supir_set_gemm_tile_n(256);
-        test_gemm(256, 256, 64, 0, false, false, false, 0, false, true);
-        test_gemm(256, 256, 256, 0, true, false, false, 0);
-        test_gemm(300, 200, 192, 0, true, true, false, 0);
-        test_gemm(1000, 328, 320, 1, true, false, true, 0);
-        test_gemm(2048, 2560, 1280, 2, true, true, false, 20000);
-        test_gemm(20000, 640, 640, 0, true, true, false, 20000);
-        test_gemm(40000, 1280, 320, 0, true, true, false, 20000);
-        test_conv(2, 32, 32, 64, 128, 0, true, true);
-        test_conv(1, 17, 23, 72, 40, 0, false, false);
-        test_conv(3, 24, 24, 320, 320, 20000, true, true);     // odd patch count: the last pair has a padding CTA
-        test_conv(2, 64, 64, 320, 320, 20000, true, true);
-        for (int bn : {160, 128}) {
-            supir_set_gemm_tile_n(bn);
-            test_gemm(256, 256, 256, 0, true, false, false, 0);
-            test_gemm(300, 200, 192, 0, true, true, false, 0);
-            test_gemm(1000, 328, 320, 1, true, false, true, 0);
-            test_gemm(2048, 2560, 1280, 2, true, true, false, 20000);
-            test_gemm(20000, 640, 640, 0, true, true, false, 20000);
-            test_conv(3, 24, 24, 320, 320, 20000, true, true);
-        }
-        supir_set_gemm_tile_n(0);
-        struct Sh { int M, N, K, act; } shapes[] = {{14336, 10240, 1280, 2}, {14336, 1280, 1280, 0}, {57344, 640, 640, 0},
-                                                    {57344, 5120, 640, 2}, {57344, 1920, 640, 0}, {57344, 640, 2560, 0},
-                                                    {229376, 320, 320, 0}, {14336, 1280, 5120, 0}, {8192, 8192, 8192, 0}};
-        for (auto& sh : shapes)
-            for (int bn : {256, 160, 128})
-                for (int pm : {0, 2}) {
-                    supir_set_gemm_pair_mode(pm);
-                    printf("pair=%d ", pm);
-                    perf_gemm(sh.M, sh.N, sh.K, sh.act, bn);
-                }
-        for (int bn : {160, 128})
-            for (int pm : {0, 2}) {
-                supir_set_gemm_pair_mode(pm);
-                printf("pair=%d ", pm);
-                perf_conv(14, 128, 128, 320, 320, bn);
-                printf("pair=%d ", pm);
-                perf_conv(14, 64, 64, 640, 640, bn);
-            }
-        for (int pm : {0, 2}) {
-            supir_set_gemm_pair_mode(pm);
-            printf("pair=%d ", pm);
-            perf_conv(14, 32, 32, 1280, 1280, 256);
-            printf("pair=%d ", pm);
-            perf_conv(14, 64, 64, 640, 640, 256);
-        }
-        supir_set_gemm_pair_mode(1);
     }
     if (what == "attnpack") {   // bf16 packing of the probabilities on the ALU pipe (0..4 of 4 pairs) instead of the XU-pipe conversion
         for (int n : {0, 2, 3, 4}) {
@@ -631,35 +506,6 @@ int main(int argc, char** argv) {
         }
         supir_set_attention_alu_pack(-1);
     }
-    if (what == "attnstagger") {   // phase offset between the two query tiles of a self-attention CTA
-        for (int st : {0, 300, 600, 900, 1200, 1600}) {
-            printf("-- tile B starts %d cycles behind tile A\n", st);
-            supir_set_attention_stagger(st);
-            perf_attention(98, 10, 4096, 4096);
-            perf_attention(98, 20, 1024, 1024);
-        }
-        supir_set_attention_stagger(600);
-        test_attention(2, 10, 1024, 1024, 500);
-        test_attention(1, 2, 333, 500, 0);
-        supir_set_attention_stagger(-1);
-    }
-    if (what == "epiperf") {     // the step's dominant GEMM shapes (batch 98) under both staged-epilogue modes
-        for (int mode : {0, 1}) {
-            printf("-- staged epilogue mode %d (%s)\n", mode, mode ? "per-warp TMA, no named barriers" : "one TMA op per 128-row chunk");
-            supir_set_gemm_epilogue_mode(mode);
-            perf_gemm_real(100352, 10240, 1280, 2, false);
-            perf_gemm_real(100352, 1280, 5120, 0, true);
-            perf_gemm_real(100352, 1280, 1280, 0, true);
-            perf_gemm_real(100352, 3840, 1280, 0, false);
-            perf_gemm_real(100352, 3840, 1280, 0, false, true);
-            perf_gemm_real(401408, 5120, 640, 2, false);
-            perf_gemm_real(401408, 640, 640, 0, true);
-            perf_gemm_real(401408, 640, 2560, 0, true);
-            perf_gemm_real(401408, 1920, 640, 0, false);
-            perf_gemm_real(401408, 1920, 640, 0, false, true);
-        }
-        supir_set_gemm_epilogue_mode(-1);
-    }
     if (what == "attnquick") {     // hang guard for a GPU session: every kernel variant once, small
         for (int emu : {0, 2}) {
             supir_set_attention_exp_emulation(emu);
@@ -667,7 +513,7 @@ int main(int argc, char** argv) {
             test_attention(2, 3, 200, 77, 0);
             test_attention(1, 2, 333, 128, 0);
             test_attention(1, 2, 333, 500, 0);
-            test_attention(40, 8, 512, 512, 200);     // 640 work items: the persistent loop wraps on every SM
+            test_attention(40, 8, 512, 512, 200);     // 1280 CTAs: several waves over the SMs
             test_attention(60, 8, 256, 77, 200);
         }
         supir_set_attention_exp_emulation(-1);
@@ -685,7 +531,7 @@ int main(int argc, char** argv) {
         test_attention(2, 10, 4096, 77, 2000);
         test_attention(3, 2, 700, 96, 0);
         test_attention(3, 2, 300, 128, 0);
-        test_attention(40, 20, 1024, 1024, 300);      // more work items than SMs: the persistent loop wraps
+        test_attention(40, 20, 1024, 1024, 300);      // many more CTAs than SMs: several waves
       }
       supir_set_attention_exp_emulation(-1);
     }
