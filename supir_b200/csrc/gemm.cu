@@ -12,8 +12,10 @@
 //                   CONV mode: A is a 4-D tensor map over the NHWC activation [B, H, W, C]; the tile's 128 rows are a
 //                   TH x TW pixel patch and the k-loop runs over (tap, 64-channel chunk); the tap shift is applied to the
 //                   TMA coordinates, and TMA's out-of-bounds zero fill IS the conv padding (no im2col buffer).
-//   warpgroups 1, 2       : wgmma consumers, rows [0, 64) and [64, 128) of the tile (m64nBNk16, fp32 accumulators in
-//                   registers, one wgmma group kept in flight); then the epilogue straight from the accumulator fragment:
+//   warpgroups 1, 2       : wgmma consumers (m64nBNk16, fp32 accumulators in registers, one wgmma group kept in flight).
+//                   BN in {160, 256}, cooperative: rows [0, 64) and [64, 128) of every tile. BN in {64, 128}, ping-pong: each
+//                   warpgroup owns alternate whole tiles, and one's epilogue runs under the other's mainloop.
+//                   Then the epilogue straight from the accumulator fragment:
 //                   +bias, +per-batch vector (timestep embedding), folded LayerNorm, SiLU / GEGLU, bf16 round, +residual,
 //                   bf16 or fp32 stores. The producer keeps filling the shared-memory ring for the next tile meanwhile.
 // Pipeline: smem full/empty mbarrier ring (TMA <-> wgmma).
@@ -59,6 +61,10 @@ struct GemmKernelParams {
     const float* ln_colsum;  // [N] row sums of the (gamma-scaled) weight matrix
 };
 
+// tile widths 64 and 128 run the ping-pong schedule (each consumer warpgroup owns whole 128 x BN tiles, BN accumulators per
+// thread); 160 and 256 run the cooperative one (both warpgroups on one tile, BN / 2 accumulators per thread)
+__host__ __device__ constexpr bool gemm_pingpong(int bn) { return bn <= 128; }
+
 template <int BN>
 struct GemmSmem {
     static constexpr int A_BYTES = BM * BK * 2;
@@ -89,10 +95,173 @@ __device__ __forceinline__ void store_pair(const GemmKernelParams& p, long long 
         else { dst[0] = __float2bfloat16_rn(v0); if (n1ok) dst[1] = __float2bfloat16_rn(v1); }
     }
 }
-__device__ __forceinline__ float2 load_res_pair(const GemmKernelParams& p, long long grow, int n, bool n1ok) {
+// residual pair (n, n + 1) as packed bf16x2 bits; a missing column n + 1 reads as 0
+__device__ __forceinline__ uint32_t load_res_bits(const GemmKernelParams& p, long long grow, int n, bool n1ok) {
     const __nv_bfloat16* src = p.residual + grow * p.ldr + n;
-    if (n1ok && ((reinterpret_cast<uintptr_t>(src) & 3) == 0)) return unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(src)));
-    return make_float2(__bfloat162float(src[0]), n1ok ? __bfloat162float(src[1]) : 0.f);
+    if (n1ok && ((reinterpret_cast<uintptr_t>(src) & 3) == 0)) return __ldg(reinterpret_cast<const unsigned int*>(src));
+    const uint32_t lo = __bfloat16_as_ushort(src[0]);
+    return n1ok ? lo | ((uint32_t)__bfloat16_as_ushort(src[1]) << 16) : lo;
+}
+
+// output row of accumulator row `row_in_tile` of m-tile `mt`: its row index in the output / residual, its image (per-batch
+// vector index) and whether it exists
+struct EpiRow {
+    long long grow;
+    int batch;
+    bool ok;
+};
+__device__ __forceinline__ EpiRow epi_row(const GemmKernelParams& p, int mt, int row_in_tile) {
+    EpiRow r;
+    if (p.conv) {
+        const int per_img = p.tiles_x * p.tiles_y;
+        const int b = mt / per_img;
+        const int t = mt % per_img;
+        const int y = (t / p.tiles_x) * p.TH + row_in_tile / p.TW;
+        const int x = (t % p.tiles_x) * p.TW + row_in_tile % p.TW;
+        r.ok = (y < p.H) && (x < p.W) && (b < p.nimg);
+        r.grow = ((long long)b * p.out_H + (long long)y * p.out_sy + p.out_oy) * p.out_W + (long long)x * p.out_sx + p.out_ox;
+        r.batch = b;
+    } else {
+        r.grow = (long long)mt * BM + row_in_tile;
+        r.ok = r.grow < p.M;
+        r.batch = p.rows_per_batch > 0 ? (int)(r.grow / p.rows_per_batch) : 0;
+    }
+    return r;
+}
+
+// Epilogue of one m64 accumulator fragment of tile (mt, nt): this thread's rows r_lo and r_lo + 8, columns 8 j + cq (+1).
+// CH > 1: the columns go in chunks of CH pairs (GEGLU: 2 groups of 32 when CH >= 8, else 1), and every global load of a chunk
+// (residual, bias, per-image vector, LN column sums) is issued before its first store, so a chunk waits for one memory latency
+// instead of one per column pair. CH == 1: one pair at a time (the cooperative 256-wide tile, see pick_bn).
+template <int BN, int CH>
+__device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const float (&acc)[BN / 2], int mt, int nt, int r_lo, int cq) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const EpiRow row = epi_row(p, mt, r_lo + 8 * h);
+        if (!row.ok) continue;
+        const long long grow = row.grow;
+        const float* rv = p.rowvec ? p.rowvec + (long long)row.batch * p.rowvec_ld : nullptr;
+        if (p.act == 2) {
+            // GEGLU: accumulator columns come in groups of 32 = [16 value | 16 gate]; this thread holds value column
+            // 8 b + cq (+1) of group g in block 4 g + b and its gate 16 columns later in block 4 g + b + 2
+            constexpr int NG = BN / 32, GCH = CH >= 8 ? 2 : 1;
+#pragma unroll
+            for (int g0 = 0; g0 < NG; g0 += GCH) {
+                if (nt * BN + g0 * 32 >= p.N) break;
+                float bx[GCH][2][4], rx[GCH][2][4];
+                uint32_t res[GCH][2];
+#pragma unroll
+                for (int gi = 0; gi < GCH; ++gi) {
+                    const int g = g0 + gi;
+                    const bool gok = g < NG && nt * BN + g * 32 < p.N;
+#pragma unroll
+                    for (int b = 0; b < 2; ++b) {
+                        const int nv = nt * BN + g * 32 + b * 8 + cq;
+                        const int offs[4] = {0, 1, 16, 17};
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            bx[gi][b][e] = (gok && p.bias) ? __ldg(p.bias + nv + offs[e]) : 0.f;
+                            rx[gi][b][e] = (gok && rv) ? __ldg(rv + nv + offs[e]) : 0.f;
+                        }
+                        const int oc = (nt * BN) / 2 + g * 16 + b * 8 + cq;
+                        res[gi][b] = (gok && p.residual) ? load_res_bits(p, grow, oc, true) : 0u;
+                    }
+                }
+#pragma unroll
+                for (int gi = 0; gi < GCH; ++gi) {
+                    const int g = g0 + gi;
+                    if (g >= NG || nt * BN + g * 32 >= p.N) break;
+#pragma unroll
+                    for (int b = 0; b < 2; ++b) {
+                        float xv0 = acc[4 * (4 * g + b) + 2 * h], xv1 = acc[4 * (4 * g + b) + 2 * h + 1];
+                        float gv0 = acc[4 * (4 * g + b + 2) + 2 * h], gv1 = acc[4 * (4 * g + b + 2) + 2 * h + 1];
+                        if (p.bias) {
+                            xv0 += bx[gi][b][0]; xv1 += bx[gi][b][1];
+                            gv0 += bx[gi][b][2]; gv1 += bx[gi][b][3];
+                        }
+                        if (rv) {
+                            xv0 += rx[gi][b][0]; xv1 += rx[gi][b][1];
+                            gv0 += rx[gi][b][2]; gv1 += rx[gi][b][3];
+                        }
+                        float o0 = bf16_round(bf16_round(xv0) * bf16_round(gelu_erf_f(bf16_round(gv0))));
+                        float o1 = bf16_round(bf16_round(xv1) * bf16_round(gelu_erf_f(bf16_round(gv1))));
+                        const int oc = (nt * BN) / 2 + g * 16 + b * 8 + cq;
+                        if (p.residual) {
+                            const float2 r = unpack_bf16x2(res[gi][b]);
+                            o0 += r.x; o1 += r.y;
+                        }
+                        store_pair(p, grow, oc, o0, o1, true);
+                    }
+                }
+            }
+        } else {
+            float ln_rs = 1.f, ln_nm = 0.f;
+            if (p.ln_stats) { const float2 st = __ldg(p.ln_stats + grow); ln_rs = st.x; ln_nm = st.y; }
+            constexpr int NJ = BN / 8;
+            // with nothing to load (QKV projections) the chunked form only adds instructions: it measured up to 35 % slower
+            if (CH == 1 || !(p.ln_stats || p.bias || rv || p.residual)) {
+#pragma unroll
+                for (int j = 0; j < NJ; ++j) {
+                    const int n = nt * BN + 8 * j + cq;
+                    if (n >= p.N) break;
+                    const bool n1ok = n + 1 < p.N;
+                    float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                    if (p.ln_stats) {
+                        v0 = fmaf(v0, ln_rs, -ln_nm * __ldg(p.ln_colsum + n));
+                        if (n1ok) v1 = fmaf(v1, ln_rs, -ln_nm * __ldg(p.ln_colsum + n + 1));
+                    }
+                    if (p.bias) { v0 += __ldg(p.bias + n); if (n1ok) v1 += __ldg(p.bias + n + 1); }
+                    if (rv) { v0 += __ldg(rv + n); if (n1ok) v1 += __ldg(rv + n + 1); }
+                    if (p.act == 1) { v0 = silu_f(bf16_round(v0)); v1 = silu_f(bf16_round(v1)); }
+                    if (p.residual) {
+                        const float2 r = unpack_bf16x2(load_res_bits(p, grow, n, n1ok));
+                        if (p.out_f32) { v0 += r.x; v1 += r.y; }
+                        else { v0 = bf16_round(v0) + r.x; v1 = bf16_round(v1) + r.y; }
+                    }
+                    store_pair(p, grow, n, v0, v1, n1ok);
+                }
+            } else
+#pragma unroll
+            for (int j0 = 0; j0 < NJ; j0 += CH) {
+                if (nt * BN + 8 * j0 >= p.N) break;
+                float cs[CH][2], bs[CH][2], rx[CH][2];
+                uint32_t res[CH];
+#pragma unroll
+                for (int c = 0; c < CH; ++c) {
+                    const int n = nt * BN + 8 * (j0 + c) + cq;
+                    const bool ok0 = j0 + c < NJ && n < p.N, ok1 = ok0 && n + 1 < p.N;
+                    cs[c][0] = (ok0 && p.ln_stats) ? __ldg(p.ln_colsum + n) : 0.f;
+                    cs[c][1] = (ok1 && p.ln_stats) ? __ldg(p.ln_colsum + n + 1) : 0.f;
+                    bs[c][0] = (ok0 && p.bias) ? __ldg(p.bias + n) : 0.f;
+                    bs[c][1] = (ok1 && p.bias) ? __ldg(p.bias + n + 1) : 0.f;
+                    rx[c][0] = (ok0 && rv) ? __ldg(rv + n) : 0.f;
+                    rx[c][1] = (ok1 && rv) ? __ldg(rv + n + 1) : 0.f;
+                    res[c] = (ok0 && p.residual) ? load_res_bits(p, grow, n, ok1) : 0u;
+                }
+#pragma unroll
+                for (int c = 0; c < CH; ++c) {
+                    const int j = j0 + c;
+                    const int n = nt * BN + 8 * j + cq;
+                    if (j >= NJ || n >= p.N) break;
+                    const bool n1ok = n + 1 < p.N;
+                    float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                    if (p.ln_stats) {
+                        v0 = fmaf(v0, ln_rs, -ln_nm * cs[c][0]);
+                        if (n1ok) v1 = fmaf(v1, ln_rs, -ln_nm * cs[c][1]);
+                    }
+                    if (p.bias) { v0 += bs[c][0]; if (n1ok) v1 += bs[c][1]; }
+                    if (rv) { v0 += rx[c][0]; if (n1ok) v1 += rx[c][1]; }
+                    if (p.act == 1) { v0 = silu_f(bf16_round(v0)); v1 = silu_f(bf16_round(v1)); }
+                    if (p.residual) {
+                        const float2 r = unpack_bf16x2(res[c]);
+                        if (p.out_f32) { v0 += r.x; v1 += r.y; }
+                        else { v0 = bf16_round(v0) + r.x; v1 = bf16_round(v1) + r.y; }
+                    }
+                    store_pair(p, grow, n, v0, v1, n1ok);
+                }
+            }
+        }
+    }
 }
 
 template <int BN>
@@ -100,6 +269,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKernelParams p) {
     using S = GemmSmem<BN>;
     constexpr int STAGES = S::STAGES;
+    constexpr bool PINGPONG = gemm_pingpong(BN);
+    // epilogue chunk (see epilogue_m64): 4 pairs when 128 accumulators per thread are live, to stay within 168 registers
+    constexpr int EPI_CH = BN == 256 ? 1 : (PINGPONG && BN == 128 ? 4 : 8);
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* smem_a = smem;
@@ -116,7 +288,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 8);   // one arrive per consumer warp
+            mbar_init(&empty_bar[s], PINGPONG ? 4 : 8);   // one arrive per warp of the warpgroup(s) consuming the stage
         }
         fence_barrier_init();
     }
@@ -167,111 +339,79 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     } else {
         asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
         // ===================== wgmma consumers + epilogue (warpgroups 1, 2) =====================
-        const int wg = (warp - 4) >> 2;                       // rows [64 wg, 64 wg + 64) of the tile
-        const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // accumulator rows r_lo and r_lo + 8
+        const int wg = (warp - 4) >> 2;
+        const int r_w = (warp & 3) * 16 + (lane >> 2);        // this thread's accumulator rows r_w and r_w + 8 of an m64 fragment
         const int cq = 2 * (lane & 3);                        // first of the two columns this thread holds per 8-column block
-        float acc[BN / 2];
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-            const int mt = p.m_fastest ? tile % p.num_m_tiles : tile / p.num_n_tiles;
-            const int nt = p.m_fastest ? tile / p.num_m_tiles : tile % p.num_n_tiles;
-            int prev = -1;
-            for (int kb = 0; kb < p.num_kb; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                const uint32_t a_addr = smem_u32(smem_a + stage * S::A_BYTES + wg * 64 * 128);
-                const uint32_t b_addr = smem_u32(smem_b + stage * S::B_BYTES);
-                wgmma_fence();
+        if constexpr (PINGPONG) {
+            // Ping-pong: warpgroup wg owns the CTA's tiles wg, wg + 2, ... (all 128 rows, two m64 fragments). Their mainloops
+            // take turns on the tensor cores through named barriers 1 and 2 (warpgroup wg waits on 1 + wg before its
+            // mainloop; the other arrives on it after finishing its own), so one warpgroup's epilogue runs under the other's
+            // mainloop. The handoff also keeps each warpgroup within one ring pass of the producer, which makes the parity
+            // waits on the full barriers unambiguous.
+            float acc[2][BN / 2];
+            int it = wg * p.num_kb;                           // ring position of this warpgroup's next k-block
+            for (int tile = blockIdx.x + wg * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x) {
+                const int mt = p.m_fastest ? tile % p.num_m_tiles : tile / p.num_n_tiles;
+                const int nt = p.m_fastest ? tile / p.num_m_tiles : tile % p.num_n_tiles;
+                if (tile != (int)blockIdx.x) named_bar_sync(1 + wg, 256);
+                int stage = it % STAGES;
+                uint32_t phase = (it / STAGES) & 1;
+                int prev = -1;
+                for (int kb = 0; kb < p.num_kb; ++kb) {
+                    mbar_wait(&full_bar[stage], phase);
+                    const uint32_t a_addr = smem_u32(smem_a + stage * S::A_BYTES);
+                    const uint32_t b_addr = smem_u32(smem_b + stage * S::B_BYTES);
+                    wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < BK / 16; ++k)       // 16 k-elements = 32 bytes inside the 128B swizzle row
-                    wgmma_tile<BN>(acc, wgmma_desc_sw128(a_addr + 32 * k), wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
-                wgmma_commit();
-                wgmma_wait<1>();                         // the previous k-block's group has retired: its slot is free
-                if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
-                prev = stage;
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                    for (int k = 0; k < BK / 16; ++k) {
+                        const uint64_t db = wgmma_desc_sw128(b_addr + 32 * k);
+                        wgmma_tile<BN>(acc[0], wgmma_desc_sw128(a_addr + 32 * k), db, (kb | k) != 0);
+                        wgmma_tile<BN>(acc[1], wgmma_desc_sw128(a_addr + 64 * 128 + 32 * k), db, (kb | k) != 0);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
+                    prev = stage;
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                }
+                wgmma_wait<0>();
+                wgmma_fence_operands(acc[0]);
+                wgmma_fence_operands(acc[1]);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                if (tile + (int)gridDim.x < num_tiles) named_bar_arrive(1 + (wg ^ 1), 256);   // the other warpgroup's turn
+                it += 2 * p.num_kb;
+                epilogue_m64<BN, EPI_CH>(p, acc[0], mt, nt, r_w, cq);
+                epilogue_m64<BN, EPI_CH>(p, acc[1], mt, nt, 64 + r_w, cq);
             }
-            wgmma_wait<0>();
-            wgmma_fence_operands(acc);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[prev]);
-
-            // ---------------- epilogue, from the accumulator fragment ----------------
+        } else {
+            // Cooperative: both warpgroups work on every tile, warpgroup wg on rows [64 wg, 64 wg + 64).
+            float acc[BN / 2];
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                const int mt = p.m_fastest ? tile % p.num_m_tiles : tile / p.num_n_tiles;
+                const int nt = p.m_fastest ? tile / p.num_m_tiles : tile % p.num_n_tiles;
+                int prev = -1;
+                for (int kb = 0; kb < p.num_kb; ++kb) {
+                    mbar_wait(&full_bar[stage], phase);
+                    const uint32_t a_addr = smem_u32(smem_a + stage * S::A_BYTES + wg * 64 * 128);
+                    const uint32_t b_addr = smem_u32(smem_b + stage * S::B_BYTES);
+                    wgmma_fence();
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int row_in_tile = r_lo + 8 * h;
-                long long grow;
-                int batch_idx;
-                bool row_ok;
-                if (p.conv) {
-                    const int per_img = p.tiles_x * p.tiles_y;
-                    const int b = mt / per_img;
-                    const int r = mt % per_img;
-                    const int y = (r / p.tiles_x) * p.TH + row_in_tile / p.TW;
-                    const int x = (r % p.tiles_x) * p.TW + row_in_tile % p.TW;
-                    row_ok = (y < p.H) && (x < p.W) && (b < p.nimg);
-                    grow = ((long long)b * p.out_H + (long long)y * p.out_sy + p.out_oy) * p.out_W + (long long)x * p.out_sx + p.out_ox;
-                    batch_idx = b;
-                } else {
-                    grow = (long long)mt * BM + row_in_tile;
-                    row_ok = grow < p.M;
-                    batch_idx = p.rows_per_batch > 0 ? (int)(grow / p.rows_per_batch) : 0;
+                    for (int k = 0; k < BK / 16; ++k)       // 16 k-elements = 32 bytes inside the 128B swizzle row
+                        wgmma_tile<BN>(acc, wgmma_desc_sw128(a_addr + 32 * k), wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
+                    wgmma_commit();
+                    wgmma_wait<1>();                         // the previous k-block's group has retired: its slot is free
+                    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
+                    prev = stage;
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
-                if (!row_ok) continue;
-                const float* rv = p.rowvec ? p.rowvec + (long long)batch_idx * p.rowvec_ld : nullptr;
-                if (p.act == 2) {
-                    // GEGLU: accumulator columns come in groups of 32 = [16 value | 16 gate]; this thread holds value column
-                    // 8 b + cq (+1) of group g in block 4 g + b and its gate 16 columns later in block 4 g + b + 2
-#pragma unroll
-                    for (int g = 0; g < BN / 32; ++g) {
-                        if (nt * BN + g * 32 >= p.N) break;
-#pragma unroll
-                        for (int b = 0; b < 2; ++b) {
-                            const int nv = nt * BN + g * 32 + b * 8 + cq;
-                            float xv0 = acc[4 * (4 * g + b) + 2 * h], xv1 = acc[4 * (4 * g + b) + 2 * h + 1];
-                            float gv0 = acc[4 * (4 * g + b + 2) + 2 * h], gv1 = acc[4 * (4 * g + b + 2) + 2 * h + 1];
-                            if (p.bias) {
-                                xv0 += __ldg(p.bias + nv); xv1 += __ldg(p.bias + nv + 1);
-                                gv0 += __ldg(p.bias + nv + 16); gv1 += __ldg(p.bias + nv + 17);
-                            }
-                            if (rv) {
-                                xv0 += __ldg(rv + nv); xv1 += __ldg(rv + nv + 1);
-                                gv0 += __ldg(rv + nv + 16); gv1 += __ldg(rv + nv + 17);
-                            }
-                            float o0 = bf16_round(bf16_round(xv0) * bf16_round(gelu_erf_f(bf16_round(gv0))));
-                            float o1 = bf16_round(bf16_round(xv1) * bf16_round(gelu_erf_f(bf16_round(gv1))));
-                            const int oc = (nt * BN) / 2 + g * 16 + b * 8 + cq;
-                            if (p.residual) {
-                                const float2 r = load_res_pair(p, grow, oc, true);
-                                o0 += r.x; o1 += r.y;
-                            }
-                            store_pair(p, grow, oc, o0, o1, true);
-                        }
-                    }
-                } else {
-                    float ln_rs = 1.f, ln_nm = 0.f;
-                    if (p.ln_stats) { const float2 st = __ldg(p.ln_stats + grow); ln_rs = st.x; ln_nm = st.y; }
-#pragma unroll
-                    for (int j = 0; j < BN / 8; ++j) {
-                        const int n = nt * BN + 8 * j + cq;
-                        if (n >= p.N) break;
-                        const bool n1ok = n + 1 < p.N;
-                        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-                        if (p.ln_stats) {
-                            v0 = fmaf(v0, ln_rs, -ln_nm * __ldg(p.ln_colsum + n));
-                            if (n1ok) v1 = fmaf(v1, ln_rs, -ln_nm * __ldg(p.ln_colsum + n + 1));
-                        }
-                        if (p.bias) { v0 += __ldg(p.bias + n); if (n1ok) v1 += __ldg(p.bias + n + 1); }
-                        if (rv) { v0 += __ldg(rv + n); if (n1ok) v1 += __ldg(rv + n + 1); }
-                        if (p.act == 1) { v0 = silu_f(bf16_round(v0)); v1 = silu_f(bf16_round(v1)); }
-                        if (p.residual) {
-                            const float2 r = load_res_pair(p, grow, n, n1ok);
-                            if (p.out_f32) { v0 += r.x; v1 += r.y; }
-                            else { v0 = bf16_round(v0) + r.x; v1 = bf16_round(v1) + r.y; }
-                        }
-                        store_pair(p, grow, n, v0, v1, n1ok);
-                    }
-                }
+                wgmma_wait<0>();
+                wgmma_fence_operands(acc);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                epilogue_m64<BN, EPI_CH>(p, acc, mt, nt, wg * 64 + r_w, cq);
             }
         }
     }
@@ -380,12 +520,13 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKerne
     p.num_n_tiles = (p.N + BN - 1) / BN;
     p.nimg = p.conv ? (int)(p.M / ((long long)p.H * p.W)) : 0;
     {
-        // tile order that minimises HBM traffic under a simple L2 model (50 MB of L2 on H100): the CTAs running together
-        // (one round) either share a W tile (m-fastest; A is re-streamed once per n-tile unless it fits L2) or share an A tile
-        // (n-fastest; W is re-streamed once per round of m-tiles unless it fits L2)
+        // tile order that minimises HBM traffic under a simple L2 model (50 MB of L2 on H100): the tiles in flight together
+        // (one round: one per SM, two under ping-pong) either share a W tile (m-fastest; A is re-streamed once per n-tile
+        // unless it fits L2) or share an A tile (n-fastest; W is re-streamed once per round of m-tiles unless it fits L2)
         const double l2 = 50e6;
         const double a_bytes = 2.0 * p.M * (p.conv ? p.Cin : p.K), w_bytes = 2.0 * p.N * p.K;
-        const double rounds_m = (double)p.num_m_tiles * p.num_n_tiles / device_sm_count();
+        const double in_flight = (double)device_sm_count() * (gemm_pingpong(BN) ? 2 : 1);
+        const double rounds_m = (double)p.num_m_tiles * p.num_n_tiles / in_flight;
         const double t_mfast = w_bytes + (a_bytes <= l2 ? a_bytes : a_bytes * p.num_n_tiles);
         const double t_nfast = a_bytes + (w_bytes <= l2 ? w_bytes : w_bytes * (rounds_m < 1 ? 1 : rounds_m));
         p.m_fastest = t_mfast < t_nfast ? 1 : 0;
@@ -399,13 +540,20 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKerne
     return SUPIR_OK;
 }
 
-// choose the N tile: minimise (rounds over the SMs) x (per-tile time). 160 divides every channel count of SUPIR
-// (320..10240) exactly; 256 has the best shared-memory traffic per flop; narrow tiles fill the machine for small M.
+// choose the N tile (and with it the schedule, see gemm_pingpong): minimise (tiles per SM) x (per-tile time), with
+//   per-tile time = per_col[bn] * bn * num_kb + overhead[bn]
+// in units of one 160-wide column-k-block. Both terms are fitted to CUDA-event timings of the denoiser step's GEMM / conv shapes
+// at every forced width on an H100 80GB HBM3 at 700 W (1980 MHz): per_col from the K = 5120 residual GEMM (M = 33792,
+// N = 1280), where the mainloop dominates; overhead from the K = 640 residual GEMM (M = 135168, N = 640), where the epilogue
+// and pipeline fill dominate. Under ping-pong (64, 128) the overhead is what the other warpgroup's mainloop does not hide.
+// GEGLU takes the 128-wide ping-pong tile: it was the fastest width on both GEGLU shapes of the step (its epilogue does the
+// most arithmetic per column and hides best under the other warpgroup's mainloop).
 static int pick_bn(const GemmKernelParams& p, int force_bn) {
     const int m_tiles = p.num_m_tiles, N = p.N, num_kb = p.num_kb;
     if (force_bn == 64 || force_bn == 128 || force_bn == 160 || force_bn == 256) return force_bn;
+    if (p.act == 2 && N >= 256) return 128;
     const int sms = device_sm_count();
-    int best = 128;
+    int best = 160;
     double best_cost = 1e30;
     const int cands[4] = {256, 160, 128, 64};
     for (int i = 0; i < 4; ++i) {
@@ -413,12 +561,9 @@ static int pick_bn(const GemmKernelParams& p, int force_bn) {
         if (bn > 64 && N <= bn / 2) continue;
         const long long tiles = (long long)m_tiles * ((N + bn - 1) / bn);
         const long long rounds = (tiles + sms - 1) / sms;
-        // MMA time of a tile ~ bn * num_kb, with a per-column penalty for narrow tiles (each k-block re-reads the whole A
-        // tile from shared memory for fewer columns); plus a per-tile overhead (pipeline fill + epilogue, which does not
-        // overlap the next tile's MMAs) of ~6 k-blocks of a 256-wide tile. Relative estimates, not measurements.
-        const double per_col = bn == 256 ? 1.0 : (bn == 160 ? 1.1 : (bn == 128 ? 1.2 : 1.6));
-        const double tile_cost = bn * per_col * num_kb + 256.0 * 6.0;
-        const double cost = rounds * tile_cost;
+        const double per_col = bn == 256 ? 1.21 : (bn == 160 ? 1.0 : (bn == 128 ? 1.34 : 1.57));
+        const double overhead = bn == 256 ? 7620.0 : (bn == 160 ? 3140.0 : (bn == 128 ? 5460.0 : 1120.0));
+        const double cost = rounds * (per_col * bn * num_kb + overhead);
         if (cost < best_cost - 1e-9) { best_cost = cost; best = bn; }
     }
     return best;
