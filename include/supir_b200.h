@@ -6,6 +6,11 @@
  *   - plain device pointers + sizes, no torch types; the caller (PyTorch host code) owns every buffer;
  *   - activations are channels-last: images [B, H, W, C] ("NHWC"), tokens [B, L, C] — the same memory;
  *   - bf16 storage unless a name says f32; statistics / softmax / accumulation are fp32 (fp64 for GroupNorm sums);
+ *   - fp16 compute mode of the diffusion networks: every entry point the networks call with 16-bit storage has an `_f16` twin
+ *     with the same signature that reads and writes fp16 (IEEE half) instead of bf16 and rounds every intermediate the bf16
+ *     function rounds to bf16 to fp16 instead (torch.autocast(float16) instead of autocast(bfloat16)); values beyond the fp16
+ *     range become +-inf, as torch's cast does. The layout-only kernels (upsample, stride-2 im2col, copy2d) move 16-bit values
+ *     of either type;
  *   - `stream` is a cudaStream_t passed as void*; every call is asynchronous on that stream and allocates nothing;
  *   - return 0 on success, negative on error; supir_last_error() returns the message (thread-local);
  *   - devices: calls run on the CALLER's current CUDA device (the one the stream belongs to). The intended deployment is one
@@ -80,6 +85,13 @@ typedef struct supir_conv_geometry {
 } supir_conv_geometry;
 int supir_conv_geom_bf16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int Hin, int Win, int Cin,
                          int Cout, const supir_conv_geometry* geom, const supir_epilogue* ep, void* stream);
+/* fp16 twins of the three above: A / W / x / Wp / residual / 16-bit out are fp16, the epilogue rounds to fp16 */
+int supir_gemm_f16(const void* A, long long lda, const void* W, long long ldw, void* out, long long ldc, int M, int N,
+                   int K, const supir_epilogue* ep, void* stream);
+int supir_conv3x3_f16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int H, int W,
+                      int Cin, int Cout, const supir_epilogue* ep, void* stream);
+int supir_conv_geom_f16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int Hin, int Win, int Cin,
+                        int Cout, const supir_conv_geometry* geom, const supir_epilogue* ep, void* stream);
 
 /* debugging / tuning knob: force the N tile (64/128/256), 0 = heuristic */
 int supir_set_gemm_tile_n(int bn);
@@ -109,6 +121,15 @@ int supir_conv3x3_small_cout(const void* x, long long ldx, const float* w, const
                              int crop_h, int crop_w, void* stream);
 /* 1x1 conv on contiguous fp32 NCHW with Cin, Cout <= 8; input pre-multiplied by in_scale (decode: 1/scale_factor).
  * Replaces quant_conv / post_quant_conv (sgm/models/autoencoder.py:297-298, 304-316). */
+/* fp16 twins: fp16 residual / out (small_cin, im2col) or fp16 x (small_cout); input and result rounded to fp16 */
+int supir_conv3x3_small_cin_f16(const float* x, long long sb, long long sc, long long sy, const float* w, const float* bias,
+                                const void* residual, long long ldr, void* out, long long ldo, int B, int H, int W, int Cin,
+                                int Cout, void* stream);
+int supir_im2col_3x3_small_cin_f16(const float* x, long long sb, long long sc, long long sy, void* out, long long ldo, int B,
+                                   int H, int W, int Cin, int KP, void* stream);
+int supir_conv3x3_small_cout_f16(const void* x, long long ldx, const float* w, const float* bias, float* out, long long ob,
+                                 long long oc, long long oy, int B, int H, int W, int Cin, int Cout, int crop_y0, int crop_x0,
+                                 int crop_h, int crop_w, void* stream);
 int supir_conv1x1_small_nchw(const float* x, const float* w, const float* bias, float* y, int B, int Cin, int Cout,
                              long long HW, float in_scale, void* stream);
 
@@ -145,6 +166,19 @@ int supir_layernorm_bf16(const void* x, long long ldx, void* y, long long ldy, l
  * pass instead of a read + write pass, and no normalised copy of the activations) */
 int supir_layernorm_stats(const void* x, long long ldx, long long rows, int C, float eps, float* stats, void* stream);
 
+/* fp16 twins of the GroupNorm / ZeroSFT / LayerNorm functions above (fp16 activations, same statistics) */
+int supir_groupnorm_stats_f16(const void* x, long long ldx, int B, int HW, int C, int groups, double* ws, long long ws_doubles,
+                              void* stream);
+int supir_groupnorm_apply_f16(const void* x, long long ldx, void* y, long long ldy, int B, int HW, int C, int groups,
+                              const double* sums, const float* mean, const float* var, const float* gamma, const float* beta,
+                              float eps, int silu, void* stream);
+int supir_zerosft_apply_f16(const void* h, long long ldh, const void* skip_raw, long long lds, int C1, const void* gamma_beta,
+                            long long ldgb, void* out, long long ldo, int B, int HW, int C, int groups, const double* sums,
+                            const float* gn_weight, const float* gn_bias, float eps, const float* control_scale, void* stream);
+int supir_layernorm_f16(const void* x, long long ldx, void* y, long long ldy, long long rows, int C, const float* gamma,
+                        const float* beta, float eps, void* stream);
+int supir_layernorm_stats_f16(const void* x, long long ldx, long long rows, int C, float eps, float* stats, void* stream);
+
 /* P = softmax(S * scale) row-wise, fp32 -> bf16 (single-head 512-dim VAE attention, model.py:187-189) */
 int supir_softmax_rows(const float* S, long long lds, void* P, long long ldp, long long rows, int cols, float scale,
                        void* stream);
@@ -157,6 +191,9 @@ int supir_softmax_rows(const float* S, long long lds, void* P, long long ldp, lo
  * ZeroCrossAttn (SUPIR_v0.py:146). */
 int supir_attention_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                          void* out, long long ldo, int B, int H, int Lq, int Lk, int head_dim, float scale, void* stream);
+/* fp16 twin (head_dim 64 only): P is rounded to fp16 before the PV product */
+int supir_attention_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
+                        void* out, long long ldo, int B, int H, int Lq, int Lk, int head_dim, float scale, void* stream);
 /* Single-head attention with a wide head over L tokens per batch element (the SDXL VAE mid-block AttnBlock, head_dim 512:
  * model.py:158-206, 209-262; tilevae.py:292-336; 128 / 256 for reduced-width VAE configurations):
  * out[b, i, 0:head_dim] = softmax(q k^T * scale) v. q/k/v/out: [B*L, ld] bf16, ld >= head_dim. Flash-style (no score matrix
@@ -168,7 +205,7 @@ int supir_attention_1head_bf16(const void* q, long long ldq, const void* k, long
 int supir_set_attention_exp_emulation(int pairs_of_4);
 /* tuning knob: how many of every 4 probability pairs are rounded / packed to bf16 with integer instructions on the ALU pipe
  * instead of cvt.rn.bf16x2.f32, which shares the XU pipe with the exponentials (0..4; environment SUPIR_B200_ATTN_ALU_PACK;
- * negative restores the default). */
+ * negative restores the default). bf16 only: it has no effect on supir_attention_f16. */
 int supir_set_attention_alu_pack(int pairs_of_4);
 
 /* ------------------------------------------------------------------------------------------------------------------ */
@@ -191,6 +228,12 @@ int supir_nhwc_bf16_to_nchw_f32(const void* x, long long ldx, float* y, int B, i
 int supir_nhwc_bf16_crop_to_nchw_f32(const void* x, long long ldx, float* y, long long ob, long long oc, long long oy, int B,
                                      int H, int W, int C, int crop_y0, int crop_x0, int crop_h, int crop_w, void* stream);
 int supir_f32_to_bf16(const float* x, void* y, long long n, void* stream);
+/* fp16 twins */
+int supir_axpy_f16(const void* a, long long lda, const void* y, long long ldy, void* out, long long ldo, long long rows,
+                   int cols, const float* scale, void* stream);
+int supir_nhwc_f16_crop_to_nchw_f32(const void* x, long long ldx, float* y, long long ob, long long oc, long long oy, int B,
+                                    int H, int W, int C, int crop_y0, int crop_x0, int crop_h, int crop_w, void* stream);
+int supir_f32_to_f16(const float* x, void* y, long long n, void* stream);
 /* timestep_embedding (sgm/modules/diffusionmodules/util.py:206-230), dim even, max_period 1e4 */
 int supir_timestep_embedding(const float* t, float* out, int B, int dim, void* stream);
 /* y = [silu]( [silu](x) @ W^T + bias ) [+ add] for B <= 16 rows (time/label embedding MLPs, per-ResBlock emb_layers:
@@ -198,6 +241,9 @@ int supir_timestep_embedding(const float* t, float* out, int B, int dim, void* s
  * final sum (emb is only ever consumed through SiLU -> Linear, so its SiLU is computed once here instead of per consumer) */
 int supir_linear_small_m(const float* x, int ldx, const void* W, const float* bias, float* y, int ldy, int B, int N, int K,
                          int silu_in, int silu_out, const float* add, int ldadd, void* stream);
+/* fp16 twin: W fp16, inputs and outputs rounded to fp16 */
+int supir_linear_small_m_f16(const float* x, int ldx, const void* W, const float* bias, float* y, int ldy, int B, int N, int K,
+                             int silu_in, int silu_out, const float* add, int ldadd, void* stream);
 /* sampler step, part 1 (sampling.py:550-556 + guiders.py:65-74 + denoiser.py:71): x_hat = x + eps*noise_mul (eps may be
  * NULL); net_in[0:n] = net_in[n:2n] = x_hat * c_in */
 int supir_edm_pre(const float* x, const float* eps, float noise_mul, float c_in, float* x_hat, float* net_in, long long n,

@@ -72,6 +72,19 @@ _SIGS = {
     "supir_activation_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_int, c_int, c_void_p],
     "supir_gaussian_latent": [c_void_p, c_void_p, c_float, c_void_p, c_int, c_int, c_ll, c_void_p],
 }
+# fp16 twins (include/supir_b200.h): same signature as the bf16 entry point they mirror
+F16_TWINS = {
+    "supir_gemm_bf16": "supir_gemm_f16", "supir_conv3x3_bf16": "supir_conv3x3_f16", "supir_conv_geom_bf16": "supir_conv_geom_f16",
+    "supir_attention_bf16": "supir_attention_f16",
+    "supir_groupnorm_stats": "supir_groupnorm_stats_f16", "supir_groupnorm_apply": "supir_groupnorm_apply_f16",
+    "supir_zerosft_apply": "supir_zerosft_apply_f16", "supir_layernorm_bf16": "supir_layernorm_f16",
+    "supir_layernorm_stats": "supir_layernorm_stats_f16",
+    "supir_conv3x3_small_cin": "supir_conv3x3_small_cin_f16", "supir_im2col_3x3_small_cin": "supir_im2col_3x3_small_cin_f16",
+    "supir_conv3x3_small_cout": "supir_conv3x3_small_cout_f16", "supir_nhwc_bf16_crop_to_nchw_f32": "supir_nhwc_f16_crop_to_nchw_f32",
+    "supir_axpy_bf16": "supir_axpy_f16", "supir_f32_to_bf16": "supir_f32_to_f16", "supir_linear_small_m": "supir_linear_small_m_f16",
+}
+_SIGS.update({f16: _SIGS[bf16] for bf16, f16 in F16_TWINS.items()})
+
 _SPECIAL = {
     "supir_last_error": ([], ctypes.c_char_p),
     "supir_version": ([], c_int),

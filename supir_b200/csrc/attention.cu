@@ -14,9 +14,11 @@
 //                             S = Q K_j^T       wgmma m64 x BKV, A and B from shared memory (both K-major)
 //                             online softmax on the S fragment in registers (row max / sum across the 4 threads of a row)
 //                             O += P V_j        wgmma m64 x 64 per value chunk, A = P straight from registers (the S
-//                                               fragment repacked to bf16: accumulator and A-operand layouts coincide),
+//                                               fragment repacked to E: accumulator and A-operand layouts coincide),
 //                                               B = V in its natural [key, channel] layout (MN-major, transposed operand)
-//                           and finally O / l stored as bf16.
+//                           and finally O / l stored as E.
+// E is the 16-bit storage type (common.cuh): Bf16, or F16 for supir_attention_f16 (head_dim 64 only), whose P is packed with
+// cvt.rn.f16x2.f32.
 // Head dim 64 (multi-head): NCH = NVC = 1, BKV = 128. The VAE's single head of 512 channels: Q stays resident (128 KB),
 // BKV = 64 keys per block (S: 32 registers per thread next to 128 of O), the 512 value columns split over two CTAs
 // (grid.y), which both compute Q K^T.
@@ -28,8 +30,8 @@
 
 namespace supir {
 
-int make_tmap_bf16(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
-                   const uint32_t* box);
+int make_tmap_16(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
+                 const uint64_t* strides_elems, const uint32_t* box);
 
 static constexpr int ATT_BM = 128;   // queries per CTA (64 per consumer warpgroup)
 static constexpr int ATT_THREADS = 384;
@@ -39,7 +41,7 @@ struct AttnParams {
     int nsplit;            // CTAs sharing one head's value columns (grid.y = heads * nsplit)
     int head_cols;         // columns of one head in q / k / v / out
     long long ldo;
-    __nv_bfloat16* out;
+    void* out;             // E
     float scale_log2;
 };
 
@@ -76,18 +78,20 @@ struct AttnSmem {
     static constexpr int TOTAL = OFF_BAR + 256 + 1024;
 };
 
-template <int BKV>
+template <int BKV, class E>
 __device__ __forceinline__ void wgmma_qk(float (&s)[BKV / 2], uint64_t da, uint64_t db, int scale_d) {
-    if constexpr (BKV == 128) wgmma_ss_n128(s, da, db, scale_d);
-    else wgmma_ss_n64(s, da, db, scale_d);
+    if constexpr (BKV == 128) wgmma_ss_n128<E>(s, da, db, scale_d);
+    else wgmma_ss_n64<E>(s, da, db, scale_d);
 }
 
 // NCH = 64-column chunks of the head dim (Q K^T depth), NVC = 64-column value chunks per CTA, BKV = keys per block,
 // EMU = exponential pairs of every 4 evaluated by ex2_emulated, ICVT = probability pairs of every 4 packed on the ALU pipe
-template <int NCH, int NVC, int BKV, int EMU, int ICVT>
+// (bf16 only: the integer packing takes the high half of the fp32 bits, which is a bf16 value and not an fp16 one)
+template <class E, int NCH, int NVC, int BKV, int EMU, int ICVT>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                        const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
+    static_assert(ICVT == 0 || !E::kF16, "ALU packing of P produces bf16 values");
     using SM = AttnSmem<NCH, NVC, BKV>;
     constexpr int SLOTS = SM::SLOTS;
     extern __shared__ uint8_t smem_raw[];
@@ -164,7 +168,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
                 const uint32_t ka = smem_u32(ring + slot * SM::SLOT);
 #pragma unroll
                 for (int kk = 0; kk < 4; ++kk)
-                    wgmma_qk<BKV>(s, wgmma_desc_sw128(qa + 32 * kk), wgmma_desc_sw128(ka + 32 * kk), (c | kk) != 0);
+                    wgmma_qk<BKV, E>(s, wgmma_desc_sw128(qa + 32 * kk), wgmma_desc_sw128(ka + 32 * kk), (c | kk) != 0);
                 if (++slot == SLOTS) { slot = 0; phase ^= 1; }
             }
             wgmma_commit();
@@ -215,7 +219,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
                     l_run[h] += e0 + e1;
                     const bool alu_pack = (ICVT == 4) || (ICVT == 2 && !(q & 1)) || (ICVT == 1 && q == 0) || (ICVT == 3 && q != 2);
                     // A fragment of k-step t/2: regs {0, 1} = keys [0, 8) of the step for rows r, r + 8; {2, 3} = keys [8, 16)
-                    pa[t >> 1][(t & 1) * 2 + h] = alu_pack ? pack_bf16x2_alu(e0, e1) : pack_bf16x2(e0, e1);
+                    pa[t >> 1][(t & 1) * 2 + h] = alu_pack ? pack_bf16x2_alu(e0, e1) : E::pack2(e0, e1);
                 }
             }
 
@@ -232,7 +236,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
                 const uint32_t va = smem_u32(ring + slot * SM::SLOT);
 #pragma unroll
                 for (int kk = 0; kk < BKV / 16; ++kk)      // 16 keys = 16 rows of 128 B = two 8-row swizzle atoms
-                    wgmma_rs_n64_tb(o[d], pa[kk], wgmma_desc_sw128(va + kk * 2048), 1);
+                    wgmma_rs_n64_tb<E>(o[d], pa[kk], wgmma_desc_sw128(va + kk * 2048), 1);
                 if (++slot == SLOTS) { slot = 0; phase ^= 1; }
             }
             wgmma_commit();
@@ -244,7 +248,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
                 for (int d = 0, sl = v_first; d < NVC; ++d, sl = (sl + 1 == SLOTS ? 0 : sl + 1)) mbar_arrive(&slot_empty[sl]);
         }
 
-        // ---- O / l -> bf16 ----
+        // ---- O / l -> E ----
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             float l = l_run[h];
@@ -253,13 +257,13 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
             const float inv = 1.f / l;
             const int qrow = q0 + r_lo + 8 * h;
             if (qrow < p.Lq) {
-                __nv_bfloat16* dst = p.out + ((long long)batch * p.Lq + qrow) * p.ldo + v_col + cq;
+                typename E::T* dst = reinterpret_cast<typename E::T*>(p.out) + ((long long)batch * p.Lq + qrow) * p.ldo + v_col + cq;
 #pragma unroll
                 for (int d = 0; d < NVC; ++d)
 #pragma unroll
                     for (int t = 0; t < 8; ++t)
                         *reinterpret_cast<uint32_t*>(dst + d * 64 + 8 * t) =
-                            pack_bf16x2(o[d][4 * t + 2 * h] * inv, o[d][4 * t + 2 * h + 1] * inv);
+                            E::pack2(o[d][4 * t + 2 * h] * inv, o[d][4 * t + 2 * h + 1] * inv);
             }
         }
     }
@@ -286,34 +290,34 @@ static int attention_emu() {
     return g_att_emu;
 }
 
-template <int NCH, int NVC, int BKV, int EMU, int ICVT>
+template <class E, int NCH, int NVC, int BKV, int EMU, int ICVT>
 static int launch_attention(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const AttnParams& p,
                             int heads, int B, cudaStream_t st) {
     using SM = AttnSmem<NCH, NVC, BKV>;
     static bool attr_set[64] = {};
     const int dslot = current_device_slot();
     if (!attr_set[dslot]) {
-        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel<NCH, NVC, BKV, EMU, ICVT>,
+        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel<E, NCH, NVC, BKV, EMU, ICVT>,
                                               cudaFuncAttributeMaxDynamicSharedMemorySize, SM::TOTAL));
         attr_set[dslot] = true;
     }
     const dim3 grid((p.Lq + ATT_BM - 1) / ATT_BM, heads * p.nsplit, B);
-    attention_wgmma_kernel<NCH, NVC, BKV, EMU, ICVT><<<grid, ATT_THREADS, SM::TOTAL, st>>>(tmQ, tmK, tmV, p);
+    attention_wgmma_kernel<E, NCH, NVC, BKV, EMU, ICVT><<<grid, ATT_THREADS, SM::TOTAL, st>>>(tmQ, tmK, tmV, p);
     count_launch();
     SUPIR_CHECK_CUDA(cudaGetLastError());
     return SUPIR_OK;
 }
 
-static int make_attention_maps(CUtensorMap* tmQ, CUtensorMap* tmK, CUtensorMap* tmV, const void* q, long long ldq, const void* k,
+static int make_attention_maps(CUtensorMapDataType dt, CUtensorMap* tmQ, CUtensorMap* tmK, CUtensorMap* tmV, const void* q, long long ldq, const void* k,
                                long long ldk, const void* v, long long ldv, uint64_t cols, uint64_t rows_q, uint64_t rows_kv,
                                uint32_t bkv) {
     int rc;
     const uint32_t box_q[2] = {64, ATT_BM}, box_kv[2] = {64, bkv};
     const uint64_t dq[2] = {cols, rows_q}, dkv[2] = {cols, rows_kv};
     const uint64_t sq[1] = {(uint64_t)ldq}, sk[1] = {(uint64_t)ldk}, sv[1] = {(uint64_t)ldv};
-    if ((rc = make_tmap_bf16(tmQ, q, 2, dq, sq, box_q))) return rc;
-    if ((rc = make_tmap_bf16(tmK, k, 2, dkv, sk, box_kv))) return rc;
-    return make_tmap_bf16(tmV, v, 2, dkv, sv, box_kv);
+    if ((rc = make_tmap_16(tmQ, dt, q, 2, dq, sq, box_q))) return rc;
+    if ((rc = make_tmap_16(tmK, dt, k, 2, dkv, sk, box_kv))) return rc;
+    return make_tmap_16(tmV, dt, v, 2, dkv, sv, box_kv);
 }
 
 }  // namespace supir
@@ -330,32 +334,57 @@ extern "C" int supir_set_attention_exp_emulation(int pairs_of_4) {
     return SUPIR_OK;
 }
 
+// head_dim-64 multi-head attention: argument checks and tensor maps shared by the bf16 and fp16 entry points
+static int attention_h64_setup(const char* who, CUtensorMapDataType dt, CUtensorMap* tmQ, CUtensorMap* tmK, CUtensorMap* tmV,
+                               AttnParams* p, const void* q, long long ldq, const void* k, long long ldk, const void* v,
+                               long long ldv, void* out, long long ldo, int B, int H, int Lq, int Lk, int head_dim, float scale) {
+    SUPIR_REQUIRE(q && k && v && out, "%s: null pointer", who);
+    SUPIR_REQUIRE(head_dim == 64, "%s: head_dim %d unsupported (64 only; the VAE's single wide head is supir_attention_1head_bf16)", who, head_dim);
+    SUPIR_REQUIRE(B > 0 && H > 0 && Lq > 0 && Lk > 0, "%s: bad shape", who);
+    SUPIR_REQUIRE(scale > 0.f, "%s: scale must be positive", who);
+    SUPIR_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0, "%s: leading dims must be multiples of 8", who);
+    int rc = make_attention_maps(dt, tmQ, tmK, tmV, q, ldq, k, ldk, v, ldv, (uint64_t)H * 64, (uint64_t)B * Lq, (uint64_t)B * Lk, 128);
+    if (rc) return rc;
+    *p = AttnParams{};
+    p->Lq = Lq; p->Lk = Lk;
+    p->nsplit = 1;
+    p->head_cols = 64;
+    p->ldo = ldo;
+    p->out = out;
+    p->scale_log2 = scale * 1.4426950408889634f;
+    return SUPIR_OK;
+}
+
 extern "C" int supir_attention_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v,
                                     long long ldv, void* out, long long ldo, int B, int H, int Lq, int Lk, int head_dim,
                                     float scale, void* stream) {
-    SUPIR_REQUIRE(q && k && v && out, "supir_attention_bf16: null pointer");
-    SUPIR_REQUIRE(head_dim == 64, "supir_attention_bf16: head_dim %d unsupported (64 only; the VAE's single wide head is supir_attention_1head_bf16)", head_dim);
-    SUPIR_REQUIRE(B > 0 && H > 0 && Lq > 0 && Lk > 0, "supir_attention_bf16: bad shape");
-    SUPIR_REQUIRE(scale > 0.f, "supir_attention_bf16: scale must be positive");
-    SUPIR_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0, "supir_attention_bf16: leading dims must be multiples of 8");
     CUtensorMap tmQ, tmK, tmV;
-    int rc = make_attention_maps(&tmQ, &tmK, &tmV, q, ldq, k, ldk, v, ldv, (uint64_t)H * 64, (uint64_t)B * Lq, (uint64_t)B * Lk, 128);
+    AttnParams p;
+    int rc = attention_h64_setup("supir_attention_bf16", Bf16::kTma, &tmQ, &tmK, &tmV, &p, q, ldq, k, ldk, v, ldv, out, ldo, B, H,
+                                 Lq, Lk, head_dim, scale);
     if (rc) return rc;
-    AttnParams p{};
-    p.Lq = Lq; p.Lk = Lk;
-    p.nsplit = 1;
-    p.head_cols = 64;
-    p.ldo = ldo;
-    p.out = reinterpret_cast<__nv_bfloat16*>(out);
-    p.scale_log2 = scale * 1.4426950408889634f;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (attention_emu() >= 2) return launch_attention<1, 1, 128, 2, 0>(tmQ, tmK, tmV, p, H, B, st);
+    if (attention_emu() >= 2) return launch_attention<Bf16, 1, 1, 128, 2, 0>(tmQ, tmK, tmV, p, H, B, st);
     switch (attention_int_pack()) {
-        case 0: return launch_attention<1, 1, 128, 0, 0>(tmQ, tmK, tmV, p, H, B, st);
-        case 1: case 2: return launch_attention<1, 1, 128, 0, 2>(tmQ, tmK, tmV, p, H, B, st);
-        case 3: return launch_attention<1, 1, 128, 0, 3>(tmQ, tmK, tmV, p, H, B, st);
-        default: return launch_attention<1, 1, 128, 0, 4>(tmQ, tmK, tmV, p, H, B, st);
+        case 0: return launch_attention<Bf16, 1, 1, 128, 0, 0>(tmQ, tmK, tmV, p, H, B, st);
+        case 1: case 2: return launch_attention<Bf16, 1, 1, 128, 0, 2>(tmQ, tmK, tmV, p, H, B, st);
+        case 3: return launch_attention<Bf16, 1, 1, 128, 0, 3>(tmQ, tmK, tmV, p, H, B, st);
+        default: return launch_attention<Bf16, 1, 1, 128, 0, 4>(tmQ, tmK, tmV, p, H, B, st);
     }
+}
+
+// fp16: the ALU-packing knob (supir_set_attention_alu_pack) has no effect here; P always goes through cvt.rn.f16x2.f32
+extern "C" int supir_attention_f16(const void* q, long long ldq, const void* k, long long ldk, const void* v,
+                                   long long ldv, void* out, long long ldo, int B, int H, int Lq, int Lk, int head_dim,
+                                   float scale, void* stream) {
+    CUtensorMap tmQ, tmK, tmV;
+    AttnParams p;
+    int rc = attention_h64_setup("supir_attention_f16", F16::kTma, &tmQ, &tmK, &tmV, &p, q, ldq, k, ldk, v, ldv, out, ldo, B, H,
+                                 Lq, Lk, head_dim, scale);
+    if (rc) return rc;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (attention_emu() >= 2) return launch_attention<F16, 1, 1, 128, 2, 0>(tmQ, tmK, tmV, p, H, B, st);
+    return launch_attention<F16, 1, 1, 128, 0, 0>(tmQ, tmK, tmV, p, H, B, st);
 }
 
 extern "C" int supir_attention_1head_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v,
@@ -367,22 +396,22 @@ extern "C" int supir_attention_1head_bf16(const void* q, long long ldq, const vo
     SUPIR_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && ldq >= head_dim && ldk >= head_dim && ldv >= head_dim && ldo >= head_dim,
                   "supir_attention_1head_bf16: leading dims must be multiples of 8 and >= head_dim");
     CUtensorMap tmQ, tmK, tmV;
-    int rc = make_attention_maps(&tmQ, &tmK, &tmV, q, ldq, k, ldk, v, ldv, (uint64_t)head_dim, (uint64_t)B * L, (uint64_t)B * L, 64);
+    int rc = make_attention_maps(Bf16::kTma, &tmQ, &tmK, &tmV, q, ldq, k, ldk, v, ldv, (uint64_t)head_dim, (uint64_t)B * L, (uint64_t)B * L, 64);
     if (rc) return rc;
     AttnParams p{};
     p.Lq = L; p.Lk = L;
     p.head_cols = head_dim;
     p.nsplit = head_dim == 512 ? 2 : 1;          // at most 256 value columns (128 fp32 registers of O per thread) per CTA
     p.ldo = ldo;
-    p.out = reinterpret_cast<__nv_bfloat16*>(out);
+    p.out = out;
     p.scale_log2 = scale * 1.4426950408889634f;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int emu = attention_emu();
     if (head_dim == 512) {
-        if (emu == 2) return launch_attention<8, 4, 64, 2, 0>(tmQ, tmK, tmV, p, 1, B, st);
-        if (emu == 4) return launch_attention<8, 4, 64, 4, 0>(tmQ, tmK, tmV, p, 1, B, st);
-        return launch_attention<8, 4, 64, 0, 0>(tmQ, tmK, tmV, p, 1, B, st);
+        if (emu == 2) return launch_attention<Bf16, 8, 4, 64, 2, 0>(tmQ, tmK, tmV, p, 1, B, st);
+        if (emu == 4) return launch_attention<Bf16, 8, 4, 64, 4, 0>(tmQ, tmK, tmV, p, 1, B, st);
+        return launch_attention<Bf16, 8, 4, 64, 0, 0>(tmQ, tmK, tmV, p, 1, B, st);
     }
-    if (head_dim == 256) return launch_attention<4, 4, 64, 0, 0>(tmQ, tmK, tmV, p, 1, B, st);
-    return launch_attention<2, 2, 64, 0, 0>(tmQ, tmK, tmV, p, 1, B, st);
+    if (head_dim == 256) return launch_attention<Bf16, 4, 4, 64, 0, 0>(tmQ, tmK, tmV, p, 1, B, st);
+    return launch_attention<Bf16, 2, 2, 64, 0, 0>(tmQ, tmK, tmV, p, 1, B, st);
 }

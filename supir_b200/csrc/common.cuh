@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -74,6 +75,49 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
     __nv_bfloat162 t = *reinterpret_cast<__nv_bfloat162*>(&u);
     return __bfloat1622float2(t);
 }
+
+__device__ __forceinline__ float f16_round(float v) { return __half2float(__float2half_rn(v)); }
+
+__device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
+    __half2 t = __floats2half2_rn(lo, hi);     // cvt.rn.f16x2.f32
+    return *reinterpret_cast<uint32_t*>(&t);
+}
+__device__ __forceinline__ float2 unpack_f16x2(uint32_t u) {
+    __half2 t = *reinterpret_cast<__half2*>(&u);
+    return __half22float2(t);
+}
+
+// ---------------------------------------------------------------------------------------------
+// 16-bit storage element types. The diffusion-network kernels are templated on one of these; everything that is not
+// storage (accumulators, statistics, softmax) stays fp32 in both. The instantiation with Bf16 is the original bf16 kernel.
+//   round       : fp32 -> nearest storage value, back as fp32 (the points where autocast rounds an intermediate tensor)
+//   pack2/unpack2: two fp32 <-> one 32-bit register of two storage values (round to nearest even)
+//   from_f/to_f : scalar conversions; bits: the raw 16 bits
+//   kF16        : selects the wgmma operand types (.f16.f16 instead of .bf16.bf16, see wgmma.cuh)
+//   kTma        : TMA data type of the tensor maps
+// ---------------------------------------------------------------------------------------------
+struct Bf16 {
+    using T = __nv_bfloat16;
+    static constexpr bool kF16 = false;
+    static constexpr CUtensorMapDataType kTma = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    static __device__ __forceinline__ float round(float v) { return bf16_round(v); }
+    static __device__ __forceinline__ uint32_t pack2(float lo, float hi) { return pack_bf16x2(lo, hi); }
+    static __device__ __forceinline__ float2 unpack2(uint32_t u) { return unpack_bf16x2(u); }
+    static __device__ __forceinline__ T from_f(float v) { return __float2bfloat16_rn(v); }
+    static __device__ __forceinline__ float to_f(T v) { return __bfloat162float(v); }
+    static __device__ __forceinline__ uint32_t bits(T v) { return __bfloat16_as_ushort(v); }
+};
+struct F16 {
+    using T = __half;
+    static constexpr bool kF16 = true;
+    static constexpr CUtensorMapDataType kTma = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    static __device__ __forceinline__ float round(float v) { return f16_round(v); }
+    static __device__ __forceinline__ uint32_t pack2(float lo, float hi) { return pack_f16x2(lo, hi); }
+    static __device__ __forceinline__ float2 unpack2(uint32_t u) { return unpack_f16x2(u); }
+    static __device__ __forceinline__ T from_f(float v) { return __float2half_rn(v); }
+    static __device__ __forceinline__ float to_f(T v) { return __half2float(v); }
+    static __device__ __forceinline__ uint32_t bits(T v) { return __half_as_ushort(v); }
+};
 
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 // erf-form GELU — F.gelu default used by GEGLU (reference sgm/modules/attention.py:91):  gelu(g) = g/2 + |g|/2 * erf(|g|/sqrt2).

@@ -60,9 +60,10 @@ __global__ void copy2d_kernel(const __nv_bfloat16* __restrict__ s, long long lds
     }
 }
 
-// out = a + y * (*scale)   (ZeroCrossAttn: x_in + x * control_scale, SUPIR_v0.py:150)
-__global__ void axpy_kernel(const __nv_bfloat16* __restrict__ a, long long lda, const __nv_bfloat16* __restrict__ y,
-                            long long ldy, __nv_bfloat16* __restrict__ o, long long ldo, long long rows, int cols,
+// out = a + y * (*scale)   (ZeroCrossAttn: x_in + x * control_scale, SUPIR_v0.py:150); E: 16-bit storage type (common.cuh)
+template <class E>
+__global__ void axpy_kernel(const typename E::T* __restrict__ a, long long lda, const typename E::T* __restrict__ y,
+                            long long ldy, typename E::T* __restrict__ o, long long ldo, long long rows, int cols,
                             const float* __restrict__ scale) {
     const float s = *scale;
     const int cv = cols >> 3;
@@ -76,8 +77,8 @@ __global__ void axpy_kernel(const __nv_bfloat16* __restrict__ a, long long lda, 
         uint32_t w[4];
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
-            const float2 fa = unpack_bf16x2(wa[t]), fy = unpack_bf16x2(wy[t]);
-            w[t] = pack_bf16x2(fa.x + bf16_round(fy.x * s), fa.y + bf16_round(fy.y * s));
+            const float2 fa = E::unpack2(wa[t]), fy = E::unpack2(wy[t]);
+            w[t] = E::pack2(fa.x + E::round(fy.x * s), fa.y + E::round(fy.y * s));
         }
         *reinterpret_cast<uint4*>(o + r * ldo + c * 8) = make_uint4(w[0], w[1], w[2], w[3]);
     }
@@ -104,8 +105,9 @@ __global__ void nhwc_bf16_to_nchw_f32_kernel(const __nv_bfloat16* __restrict__ x
         y[i] = __bfloat162float(x[(b * HW + p) * ldx + c]);
     }
 }
-// crop window of an NHWC bf16 tile -> fp32 NCHW view with arbitrary strides (tiled-VAE paste; UNet output)
-__global__ void nhwc_bf16_crop_to_nchw_f32_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, float* __restrict__ y,
+// crop window of an NHWC 16-bit tile -> fp32 NCHW view with arbitrary strides (tiled-VAE paste; UNet output)
+template <class E>
+__global__ void nhwc_crop_to_nchw_f32_kernel(const typename E::T* __restrict__ x, long long ldx, float* __restrict__ y,
                                                   long long ob, long long oc, long long oy, int B, int H, int W, int C,
                                                   int cy0, int cx0, int ch, int cw) {
     const long long total = (long long)B * C * ch * cw;
@@ -115,12 +117,13 @@ __global__ void nhwc_bf16_crop_to_nchw_f32_kernel(const __nv_bfloat16* __restric
         const int yo = (int)(r % ch); r /= ch;
         const int c = (int)(r % C);
         const int b = (int)(r / C);
-        y[b * ob + c * oc + yo * oy + xo] = __bfloat162float(x[(((long long)b * H + yo + cy0) * W + xo + cx0) * ldx + c]);
+        y[b * ob + c * oc + yo * oy + xo] = E::to_f(x[(((long long)b * H + yo + cy0) * W + xo + cx0) * ldx + c]);
     }
 }
-__global__ void f32_to_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, long long n) {
+template <class E>
+__global__ void f32_to_16_kernel(const float* __restrict__ x, typename E::T* __restrict__ y, long long n) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        y[i] = __float2bfloat16_rn(x[i]);
+        y[i] = E::from_f(x[i]);
 }
 
 // sinusoidal timestep embedding (sgm/modules/diffusionmodules/util.py:206-230): [cos(t f_i) | sin(t f_i)], f_i = exp(-ln(1e4) i / half)
@@ -136,9 +139,9 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, float* __
 }
 
 // y[b, n] = act_out( sum_k act_in(x[b, k]) * W[n, k] + bias[n] )  for tiny batch (M <= 8): one warp per output column.
-// Inputs/outputs are rounded to bf16 at the points autocast rounds them (Linear inputs and outputs).
-template <int MAXB>
-__global__ void linear_small_m_kernel(const float* __restrict__ x, int ldx, const __nv_bfloat16* __restrict__ W,
+// Inputs/outputs are rounded to E at the points autocast rounds them (Linear inputs and outputs).
+template <int MAXB, class E>
+__global__ void linear_small_m_kernel(const float* __restrict__ x, int ldx, const typename E::T* __restrict__ W,
                                       const float* __restrict__ bias, float* __restrict__ y, int ldy, int B, int N,
                                       int K, int silu_in, int silu_out, const float* __restrict__ add, int ldadd) {
     const int n = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -147,14 +150,14 @@ __global__ void linear_small_m_kernel(const float* __restrict__ x, int ldx, cons
     float acc[MAXB];
 #pragma unroll
     for (int b = 0; b < MAXB; ++b) acc[b] = 0.f;
-    const __nv_bfloat16* w = W + (long long)n * K;
+    const typename E::T* w = W + (long long)n * K;
     for (int k0 = lane * 8; k0 < K; k0 += 256) {
         const uint4 u = __ldg(reinterpret_cast<const uint4*>(w + k0));
         const uint32_t ww[4] = {u.x, u.y, u.z, u.w};
         float wf[8];
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
-            const float2 f = unpack_bf16x2(ww[t]);
+            const float2 f = E::unpack2(ww[t]);
             wf[2 * t] = f.x; wf[2 * t + 1] = f.y;
         }
 #pragma unroll
@@ -163,8 +166,8 @@ __global__ void linear_small_m_kernel(const float* __restrict__ x, int ldx, cons
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     float xv = x[b * ldx + k0 + j];
-                    if (silu_in) xv = silu_f(bf16_round(xv));
-                    acc[b] += bf16_round(xv) * wf[j];
+                    if (silu_in) xv = silu_f(E::round(xv));
+                    acc[b] += E::round(xv) * wf[j];
                 }
             }
         }
@@ -174,10 +177,10 @@ __global__ void linear_small_m_kernel(const float* __restrict__ x, int ldx, cons
         if (b < B) {
             float v = warp_sum(acc[b]);
             if (lane == 0) {
-                v = bf16_round(v + (bias ? bias[n] : 0.f));
-                if (silu_out & 1) v = bf16_round(silu_f(v));
-                if (add) v = bf16_round(v + add[b * ldadd + n]);
-                if (silu_out & 2) v = bf16_round(silu_f(v));     // SiLU of the sum: what every consumer of `emb` applies first
+                v = E::round(v + (bias ? bias[n] : 0.f));
+                if (silu_out & 1) v = E::round(silu_f(v));
+                if (add) v = E::round(v + add[b * ldadd + n]);
+                if (silu_out & 2) v = E::round(silu_f(v));     // SiLU of the sum: what every consumer of `emb` applies first
                 y[b * ldy + n] = v;
             }
         }
@@ -303,6 +306,8 @@ using namespace supir;
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 #define BF(p) reinterpret_cast<__nv_bfloat16*>(p)
 #define CBF(p) reinterpret_cast<const __nv_bfloat16*>(p)
+#define H16(p) reinterpret_cast<__half*>(p)
+#define CH(p) reinterpret_cast<const __half*>(p)
 #define DONE()                              \
     do {                                    \
         count_launch();                     \
@@ -336,8 +341,16 @@ extern "C" int supir_copy2d_bf16(const void* src, long long lds, void* dst, long
 extern "C" int supir_axpy_bf16(const void* a, long long lda, const void* y, long long ldy, void* out, long long ldo,
                                long long rows, int cols, const float* scale, void* stream) {
     SUPIR_REQUIRE(a && y && out && scale && cols % 8 == 0, "supir_axpy_bf16: bad args");
-    axpy_kernel<<<blocks_for(rows * (cols >> 3), 256), 256, 0, ST(stream)>>>(CBF(a), lda, CBF(y), ldy, BF(out), ldo, rows,
-                                                                             cols, scale);
+    axpy_kernel<Bf16><<<blocks_for(rows * (cols >> 3), 256), 256, 0, ST(stream)>>>(CBF(a), lda, CBF(y), ldy, BF(out), ldo, rows,
+                                                                                   cols, scale);
+    DONE();
+}
+
+extern "C" int supir_axpy_f16(const void* a, long long lda, const void* y, long long ldy, void* out, long long ldo,
+                              long long rows, int cols, const float* scale, void* stream) {
+    SUPIR_REQUIRE(a && y && out && scale && cols % 8 == 0, "supir_axpy_f16: bad args");
+    axpy_kernel<F16><<<blocks_for(rows * (cols >> 3), 256), 256, 0, ST(stream)>>>(CH(a), lda, CH(y), ldy, H16(out), ldo, rows,
+                                                                                  cols, scale);
     DONE();
 }
 
@@ -359,14 +372,31 @@ extern "C" int supir_nhwc_bf16_crop_to_nchw_f32(const void* x, long long ldx, fl
     SUPIR_REQUIRE(x && y, "supir_nhwc_bf16_crop_to_nchw_f32: null pointer");
     SUPIR_REQUIRE(crop_y0 >= 0 && crop_x0 >= 0 && crop_h > 0 && crop_w > 0 && crop_y0 + crop_h <= H && crop_x0 + crop_w <= W,
                   "supir_nhwc_bf16_crop_to_nchw_f32: crop window outside the tile");
-    nhwc_bf16_crop_to_nchw_f32_kernel<<<blocks_for((long long)B * C * crop_h * crop_w, 256), 256, 0, ST(stream)>>>(
+    nhwc_crop_to_nchw_f32_kernel<Bf16><<<blocks_for((long long)B * C * crop_h * crop_w, 256), 256, 0, ST(stream)>>>(
         CBF(x), ldx, y, ob, oc, oy, B, H, W, C, crop_y0, crop_x0, crop_h, crop_w);
+    DONE();
+}
+
+extern "C" int supir_nhwc_f16_crop_to_nchw_f32(const void* x, long long ldx, float* y, long long ob, long long oc, long long oy,
+                                               int B, int H, int W, int C, int crop_y0, int crop_x0, int crop_h, int crop_w,
+                                               void* stream) {
+    SUPIR_REQUIRE(x && y, "supir_nhwc_f16_crop_to_nchw_f32: null pointer");
+    SUPIR_REQUIRE(crop_y0 >= 0 && crop_x0 >= 0 && crop_h > 0 && crop_w > 0 && crop_y0 + crop_h <= H && crop_x0 + crop_w <= W,
+                  "supir_nhwc_f16_crop_to_nchw_f32: crop window outside the tile");
+    nhwc_crop_to_nchw_f32_kernel<F16><<<blocks_for((long long)B * C * crop_h * crop_w, 256), 256, 0, ST(stream)>>>(
+        CH(x), ldx, y, ob, oc, oy, B, H, W, C, crop_y0, crop_x0, crop_h, crop_w);
     DONE();
 }
 
 extern "C" int supir_f32_to_bf16(const float* x, void* y, long long n, void* stream) {
     SUPIR_REQUIRE(x && y && n > 0, "supir_f32_to_bf16: bad args");
-    f32_to_bf16_kernel<<<blocks_for(n, 256), 256, 0, ST(stream)>>>(x, BF(y), n);
+    f32_to_16_kernel<Bf16><<<blocks_for(n, 256), 256, 0, ST(stream)>>>(x, BF(y), n);
+    DONE();
+}
+
+extern "C" int supir_f32_to_f16(const float* x, void* y, long long n, void* stream) {
+    SUPIR_REQUIRE(x && y && n > 0, "supir_f32_to_f16: bad args");
+    f32_to_16_kernel<F16><<<blocks_for(n, 256), 256, 0, ST(stream)>>>(x, H16(y), n);
     DONE();
 }
 
@@ -377,18 +407,30 @@ extern "C" int supir_timestep_embedding(const float* t, float* out, int B, int d
     DONE();
 }
 
-extern "C" int supir_linear_small_m(const float* x, int ldx, const void* W, const float* bias, float* y, int ldy, int B,
-                                    int N, int K, int silu_in, int silu_out, const float* add, int ldadd, void* stream) {
-    SUPIR_REQUIRE(x && W && y && B >= 1 && B <= 16 && K % 8 == 0, "supir_linear_small_m: bad args (B=%d K=%d)", B, K);
+template <class E>
+static int linear_small_m_impl(const char* who, const float* x, int ldx, const void* W, const float* bias, float* y, int ldy, int B,
+                               int N, int K, int silu_in, int silu_out, const float* add, int ldadd, void* stream) {
+    SUPIR_REQUIRE(x && W && y && B >= 1 && B <= 16 && K % 8 == 0, "%s: bad args (B=%d K=%d)", who, B, K);
     const int warps = 8;
     const unsigned blocks = (N + warps - 1) / warps;
+    const typename E::T* w = reinterpret_cast<const typename E::T*>(W);
     if (B <= 4)
-        linear_small_m_kernel<4><<<blocks, warps * 32, 0, ST(stream)>>>(x, ldx, CBF(W), bias, y, ldy, B, N, K, silu_in,
-                                                                        silu_out, add, ldadd);
+        linear_small_m_kernel<4, E><<<blocks, warps * 32, 0, ST(stream)>>>(x, ldx, w, bias, y, ldy, B, N, K, silu_in,
+                                                                           silu_out, add, ldadd);
     else
-        linear_small_m_kernel<16><<<blocks, warps * 32, 0, ST(stream)>>>(x, ldx, CBF(W), bias, y, ldy, B, N, K, silu_in,
-                                                                         silu_out, add, ldadd);
+        linear_small_m_kernel<16, E><<<blocks, warps * 32, 0, ST(stream)>>>(x, ldx, w, bias, y, ldy, B, N, K, silu_in,
+                                                                            silu_out, add, ldadd);
     DONE();
+}
+
+extern "C" int supir_linear_small_m(const float* x, int ldx, const void* W, const float* bias, float* y, int ldy, int B,
+                                    int N, int K, int silu_in, int silu_out, const float* add, int ldadd, void* stream) {
+    return linear_small_m_impl<Bf16>("supir_linear_small_m", x, ldx, W, bias, y, ldy, B, N, K, silu_in, silu_out, add, ldadd, stream);
+}
+
+extern "C" int supir_linear_small_m_f16(const float* x, int ldx, const void* W, const float* bias, float* y, int ldy, int B,
+                                        int N, int K, int silu_in, int silu_out, const float* add, int ldadd, void* stream) {
+    return linear_small_m_impl<F16>("supir_linear_small_m_f16", x, ldx, W, bias, y, ldy, B, N, K, silu_in, silu_out, add, ldadd, stream);
 }
 
 extern "C" int supir_edm_pre(const float* x, const float* eps, float noise_mul, float c_in, float* x_hat, float* net_in,

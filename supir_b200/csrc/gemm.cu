@@ -1,6 +1,9 @@
 // supir_b200 — K2/K3/K4 of SURVEY.md §2a: Linear, conv1x1 and conv3x3 (implicit GEMM) on Hopper wgmma.
 //
-//   out[m, n] = epilogue( sum_k A[m, k] * W[n, k] )          bf16 x bf16 -> fp32 (registers) -> bf16/fp32
+//   out[m, n] = epilogue( sum_k A[m, k] * W[n, k] )          E x E -> fp32 (registers) -> E/fp32
+//
+// E is the 16-bit storage type (common.cuh): Bf16 (supir_gemm_bf16 ...) or F16 (the _f16 twins). Every rounding point of
+// the epilogue rounds to E.
 //
 // Replaces, on the sampling path of the reference: nn.Linear (sgm/modules/attention.py:213-218,87,106,587,611),
 // nn.Conv2d 1x1 (openaimodel.py:317, SUPIR_v0.py:48,87, model.py:124-126,164-175) and nn.Conv2d 3x3 stride 1 pad 1
@@ -49,7 +52,7 @@ struct GemmKernelParams {
     const float* rowvec;
     int rows_per_batch;
     int rowvec_ld;
-    const __nv_bfloat16* residual;
+    const void* residual;     // E [M, ldr]
     long long ldr;
     int act;
     void* out;
@@ -75,32 +78,34 @@ struct GemmSmem {
     static constexpr int TOTAL = STAGES * STAGE_BYTES + BAR_BYTES + 1024;  // +1024 alignment slack
 };
 
-template <int BN>
+template <int BN, class E>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
-    if constexpr (BN == 256) wgmma_ss_n256(d, da, db, scale_d);
-    else if constexpr (BN == 160) wgmma_ss_n160(d, da, db, scale_d);
-    else if constexpr (BN == 128) wgmma_ss_n128(d, da, db, scale_d);
-    else wgmma_ss_n64(d, da, db, scale_d);
+    if constexpr (BN == 256) wgmma_ss_n256<E>(d, da, db, scale_d);
+    else if constexpr (BN == 160) wgmma_ss_n160<E>(d, da, db, scale_d);
+    else if constexpr (BN == 128) wgmma_ss_n128<E>(d, da, db, scale_d);
+    else wgmma_ss_n64<E>(d, da, db, scale_d);
 }
 
 // two adjacent output columns (n, n + 1) of one row; `n1ok`: column n + 1 exists
+template <class E>
 __device__ __forceinline__ void store_pair(const GemmKernelParams& p, long long grow, int n, float v0, float v1, bool n1ok) {
     if (p.out_f32) {
         float* dst = reinterpret_cast<float*>(p.out) + grow * p.ldc + n;
         if (n1ok && ((reinterpret_cast<uintptr_t>(dst) & 7) == 0)) { *reinterpret_cast<float2*>(dst) = make_float2(v0, v1); }
         else { dst[0] = v0; if (n1ok) dst[1] = v1; }
     } else {
-        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out) + grow * p.ldc + n;
-        if (n1ok && ((reinterpret_cast<uintptr_t>(dst) & 3) == 0)) { *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(v0, v1); }
-        else { dst[0] = __float2bfloat16_rn(v0); if (n1ok) dst[1] = __float2bfloat16_rn(v1); }
+        typename E::T* dst = reinterpret_cast<typename E::T*>(p.out) + grow * p.ldc + n;
+        if (n1ok && ((reinterpret_cast<uintptr_t>(dst) & 3) == 0)) { *reinterpret_cast<uint32_t*>(dst) = E::pack2(v0, v1); }
+        else { dst[0] = E::from_f(v0); if (n1ok) dst[1] = E::from_f(v1); }
     }
 }
-// residual pair (n, n + 1) as packed bf16x2 bits; a missing column n + 1 reads as 0
+// residual pair (n, n + 1) as the packed bits of two E values; a missing column n + 1 reads as 0
+template <class E>
 __device__ __forceinline__ uint32_t load_res_bits(const GemmKernelParams& p, long long grow, int n, bool n1ok) {
-    const __nv_bfloat16* src = p.residual + grow * p.ldr + n;
+    const typename E::T* src = reinterpret_cast<const typename E::T*>(p.residual) + grow * p.ldr + n;
     if (n1ok && ((reinterpret_cast<uintptr_t>(src) & 3) == 0)) return __ldg(reinterpret_cast<const unsigned int*>(src));
-    const uint32_t lo = __bfloat16_as_ushort(src[0]);
-    return n1ok ? lo | ((uint32_t)__bfloat16_as_ushort(src[1]) << 16) : lo;
+    const uint32_t lo = E::bits(src[0]);
+    return n1ok ? lo | (E::bits(src[1]) << 16) : lo;
 }
 
 // output row of accumulator row `row_in_tile` of m-tile `mt`: its row index in the output / residual, its image (per-batch
@@ -133,7 +138,7 @@ __device__ __forceinline__ EpiRow epi_row(const GemmKernelParams& p, int mt, int
 // CH > 1: the columns go in chunks of CH pairs (GEGLU: 2 groups of 32 when CH >= 8, else 1), and every global load of a chunk
 // (residual, bias, per-image vector, LN column sums) is issued before its first store, so a chunk waits for one memory latency
 // instead of one per column pair. CH == 1: one pair at a time (the cooperative 256-wide tile, see pick_bn).
-template <int BN, int CH>
+template <int BN, int CH, class E>
 __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const float (&acc)[BN / 2], int mt, int nt, int r_lo, int cq) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -164,7 +169,7 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
                             rx[gi][b][e] = (gok && rv) ? __ldg(rv + nv + offs[e]) : 0.f;
                         }
                         const int oc = (nt * BN) / 2 + g * 16 + b * 8 + cq;
-                        res[gi][b] = (gok && p.residual) ? load_res_bits(p, grow, oc, true) : 0u;
+                        res[gi][b] = (gok && p.residual) ? load_res_bits<E>(p, grow, oc, true) : 0u;
                     }
                 }
 #pragma unroll
@@ -183,14 +188,14 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
                             xv0 += rx[gi][b][0]; xv1 += rx[gi][b][1];
                             gv0 += rx[gi][b][2]; gv1 += rx[gi][b][3];
                         }
-                        float o0 = bf16_round(bf16_round(xv0) * bf16_round(gelu_erf_f(bf16_round(gv0))));
-                        float o1 = bf16_round(bf16_round(xv1) * bf16_round(gelu_erf_f(bf16_round(gv1))));
+                        float o0 = E::round(E::round(xv0) * E::round(gelu_erf_f(E::round(gv0))));
+                        float o1 = E::round(E::round(xv1) * E::round(gelu_erf_f(E::round(gv1))));
                         const int oc = (nt * BN) / 2 + g * 16 + b * 8 + cq;
                         if (p.residual) {
-                            const float2 r = unpack_bf16x2(res[gi][b]);
+                            const float2 r = E::unpack2(res[gi][b]);
                             o0 += r.x; o1 += r.y;
                         }
-                        store_pair(p, grow, oc, o0, o1, true);
+                        store_pair<E>(p, grow, oc, o0, o1, true);
                     }
                 }
             }
@@ -212,13 +217,13 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
                     }
                     if (p.bias) { v0 += __ldg(p.bias + n); if (n1ok) v1 += __ldg(p.bias + n + 1); }
                     if (rv) { v0 += __ldg(rv + n); if (n1ok) v1 += __ldg(rv + n + 1); }
-                    if (p.act == 1) { v0 = silu_f(bf16_round(v0)); v1 = silu_f(bf16_round(v1)); }
+                    if (p.act == 1) { v0 = silu_f(E::round(v0)); v1 = silu_f(E::round(v1)); }
                     if (p.residual) {
-                        const float2 r = unpack_bf16x2(load_res_bits(p, grow, n, n1ok));
+                        const float2 r = E::unpack2(load_res_bits<E>(p, grow, n, n1ok));
                         if (p.out_f32) { v0 += r.x; v1 += r.y; }
-                        else { v0 = bf16_round(v0) + r.x; v1 = bf16_round(v1) + r.y; }
+                        else { v0 = E::round(v0) + r.x; v1 = E::round(v1) + r.y; }
                     }
-                    store_pair(p, grow, n, v0, v1, n1ok);
+                    store_pair<E>(p, grow, n, v0, v1, n1ok);
                 }
             } else
 #pragma unroll
@@ -236,7 +241,7 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
                     bs[c][1] = (ok1 && p.bias) ? __ldg(p.bias + n + 1) : 0.f;
                     rx[c][0] = (ok0 && rv) ? __ldg(rv + n) : 0.f;
                     rx[c][1] = (ok1 && rv) ? __ldg(rv + n + 1) : 0.f;
-                    res[c] = (ok0 && p.residual) ? load_res_bits(p, grow, n, ok1) : 0u;
+                    res[c] = (ok0 && p.residual) ? load_res_bits<E>(p, grow, n, ok1) : 0u;
                 }
 #pragma unroll
                 for (int c = 0; c < CH; ++c) {
@@ -251,20 +256,20 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
                     }
                     if (p.bias) { v0 += bs[c][0]; if (n1ok) v1 += bs[c][1]; }
                     if (rv) { v0 += rx[c][0]; if (n1ok) v1 += rx[c][1]; }
-                    if (p.act == 1) { v0 = silu_f(bf16_round(v0)); v1 = silu_f(bf16_round(v1)); }
+                    if (p.act == 1) { v0 = silu_f(E::round(v0)); v1 = silu_f(E::round(v1)); }
                     if (p.residual) {
-                        const float2 r = unpack_bf16x2(res[c]);
+                        const float2 r = E::unpack2(res[c]);
                         if (p.out_f32) { v0 += r.x; v1 += r.y; }
-                        else { v0 = bf16_round(v0) + r.x; v1 = bf16_round(v1) + r.y; }
+                        else { v0 = E::round(v0) + r.x; v1 = E::round(v1) + r.y; }
                     }
-                    store_pair(p, grow, n, v0, v1, n1ok);
+                    store_pair<E>(p, grow, n, v0, v1, n1ok);
                 }
             }
         }
     }
 }
 
-template <int BN>
+template <int BN, class E>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKernelParams p) {
     using S = GemmSmem<BN>;
@@ -365,8 +370,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
                     for (int k = 0; k < BK / 16; ++k) {
                         const uint64_t db = wgmma_desc_sw128(b_addr + 32 * k);
-                        wgmma_tile<BN>(acc[0], wgmma_desc_sw128(a_addr + 32 * k), db, (kb | k) != 0);
-                        wgmma_tile<BN>(acc[1], wgmma_desc_sw128(a_addr + 64 * 128 + 32 * k), db, (kb | k) != 0);
+                        wgmma_tile<BN, E>(acc[0], wgmma_desc_sw128(a_addr + 32 * k), db, (kb | k) != 0);
+                        wgmma_tile<BN, E>(acc[1], wgmma_desc_sw128(a_addr + 64 * 128 + 32 * k), db, (kb | k) != 0);
                     }
                     wgmma_commit();
                     wgmma_wait<1>();
@@ -381,8 +386,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 if (lane == 0) mbar_arrive(&empty_bar[prev]);
                 if (tile + (int)gridDim.x < num_tiles) named_bar_arrive(1 + (wg ^ 1), 256);   // the other warpgroup's turn
                 it += 2 * p.num_kb;
-                epilogue_m64<BN, EPI_CH>(p, acc[0], mt, nt, r_w, cq);
-                epilogue_m64<BN, EPI_CH>(p, acc[1], mt, nt, 64 + r_w, cq);
+                epilogue_m64<BN, EPI_CH, E>(p, acc[0], mt, nt, r_w, cq);
+                epilogue_m64<BN, EPI_CH, E>(p, acc[1], mt, nt, 64 + r_w, cq);
             }
         } else {
             // Cooperative: both warpgroups work on every tile, warpgroup wg on rows [64 wg, 64 wg + 64).
@@ -400,7 +405,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     wgmma_fence();
 #pragma unroll
                     for (int k = 0; k < BK / 16; ++k)       // 16 k-elements = 32 bytes inside the 128B swizzle row
-                        wgmma_tile<BN>(acc, wgmma_desc_sw128(a_addr + 32 * k), wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
+                        wgmma_tile<BN, E>(acc, wgmma_desc_sw128(a_addr + 32 * k), wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
                     wgmma_commit();
                     wgmma_wait<1>();                         // the previous k-block's group has retired: its slot is free
                     if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
@@ -411,7 +416,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 wgmma_fence_operands(acc);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty_bar[prev]);
-                epilogue_m64<BN, EPI_CH>(p, acc, mt, nt, wg * 64 + r_w, cq);
+                epilogue_m64<BN, EPI_CH, E>(p, acc, mt, nt, wg * 64 + r_w, cq);
             }
         }
     }
@@ -438,9 +443,10 @@ static PFN_tmapEncodeTiled get_encode_fn() {
     return fn;
 }
 
-// rank-N bf16 tensor map with 128B swizzle; dims/strides innermost first; strides in ELEMENTS for dims 1..rank-1
-int make_tmap_bf16_sw(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
-                      const uint32_t* box, int swizzle_bytes) {
+// rank-N tensor map of 16-bit elements (bf16 or fp16: `dt`); dims/strides innermost first; strides in ELEMENTS for
+// dims 1..rank-1
+static int make_tmap_16_sw(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
+                           const uint64_t* strides_elems, const uint32_t* box, int swizzle_bytes) {
     PFN_tmapEncodeTiled fn = get_encode_fn();
     if (!fn) return set_error(SUPIR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
     cuuint64_t gdim[5], gstr[4];
@@ -459,21 +465,32 @@ int make_tmap_bf16_sw(CUtensorMap* m, const void* base, int rank, const uint64_t
     const CUtensorMapSwizzle sw = swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
                                   : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
                                   : swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE;
-    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
+    CUresult r = fn(m, dt, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return set_error(SUPIR_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
     return SUPIR_OK;
 }
 
+int make_tmap_bf16_sw(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
+                      const uint32_t* box, int swizzle_bytes) {
+    return make_tmap_16_sw(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_elems, box, swizzle_bytes);
+}
+
+// 128B-swizzled map of a GEMM / attention operand
+int make_tmap_16(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
+                 const uint64_t* strides_elems, const uint32_t* box) {
+    return make_tmap_16_sw(m, dt, base, rank, dims, strides_elems, box, 128);
+}
+
 int make_tmap_bf16(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
                    const uint32_t* box) {
-    return make_tmap_bf16_sw(m, base, rank, dims, strides_elems, box, 128);
+    return make_tmap_16(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_elems, box);
 }
 
 // same with traversal strides (elementStrides): the box spans box[i] tensor elements of dimension i and delivers every
 // elem_strides[i]-th of them, densely packed (a stride-2 convolution's input patch)
-int make_tmap_bf16_strided(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
-                           const uint32_t* box, const uint32_t* elem_strides) {
+static int make_tmap_16_strided(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
+                                const uint64_t* strides_elems, const uint32_t* box, const uint32_t* elem_strides) {
     PFN_tmapEncodeTiled fn = get_encode_fn();
     if (!fn) return set_error(SUPIR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
     cuuint64_t gdim[5], gstr[4];
@@ -483,7 +500,7 @@ int make_tmap_bf16_strided(CUtensorMap* m, const void* base, int rank, const uin
     if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return set_error(SUPIR_ERR_INVALID, "TMA base address %p is not 16-byte aligned", base);
     for (int i = 0; i + 1 < rank; ++i)
         if (gstr[i] % 16 != 0) return set_error(SUPIR_ERR_INVALID, "TMA stride %d (%llu B) not a multiple of 16", i, (unsigned long long)gstr[i]);
-    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
+    CUresult r = fn(m, dt, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return set_error(SUPIR_ERR_CUDA, "cuTensorMapEncodeTiled (strided) failed with CUresult %d", (int)r);
     return SUPIR_OK;
@@ -508,13 +525,13 @@ int device_sm_count() {
 
 extern int g_force_bn;
 
-template <int BN>
+template <int BN, class E>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKernelParams p, cudaStream_t st) {
     using S = GemmSmem<BN>;
     static bool attr_set[64] = {};
     const int dslot = current_device_slot();
     if (!attr_set[dslot]) {
-        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel<BN, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
         attr_set[dslot] = true;
     }
     p.num_n_tiles = (p.N + BN - 1) / BN;
@@ -534,7 +551,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKerne
     const int tiles = p.num_m_tiles * p.num_n_tiles;
     const int slots = device_sm_count();
     const int grid = tiles < slots ? tiles : slots;
-    gemm_wgmma_kernel<BN><<<grid, GEMM_THREADS, S::TOTAL, st>>>(tmA, tmB, p);
+    gemm_wgmma_kernel<BN, E><<<grid, GEMM_THREADS, S::TOTAL, st>>>(tmA, tmB, p);
     count_launch();
     SUPIR_CHECK_CUDA(cudaGetLastError());
     return SUPIR_OK;
@@ -571,12 +588,13 @@ static int pick_bn(const GemmKernelParams& p, int force_bn) {
 
 int g_force_bn = 0;
 
+template <class E>
 static int run_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKernelParams& p, cudaStream_t st) {
     const int bn = pick_bn(p, g_force_bn);
-    if (bn == 256) return launch_gemm<256>(tmA, tmB, p, st);
-    if (bn == 160) return launch_gemm<160>(tmA, tmB, p, st);
-    if (bn == 128) return launch_gemm<128>(tmA, tmB, p, st);
-    return launch_gemm<64>(tmA, tmB, p, st);
+    if (bn == 256) return launch_gemm<256, E>(tmA, tmB, p, st);
+    if (bn == 160) return launch_gemm<160, E>(tmA, tmB, p, st);
+    if (bn == 128) return launch_gemm<128, E>(tmA, tmB, p, st);
+    return launch_gemm<64, E>(tmA, tmB, p, st);
 }
 
 static int fill_epilogue(GemmKernelParams& p, const supir_epilogue* ep, int N) {
@@ -593,7 +611,7 @@ static int fill_epilogue(GemmKernelParams& p, const supir_epilogue* ep, int N) {
         p.rowvec = ep->rowvec;
         p.rows_per_batch = ep->rows_per_batch;
         p.rowvec_ld = ep->rowvec_ld > 0 ? ep->rowvec_ld : N;
-        p.residual = reinterpret_cast<const __nv_bfloat16*>(ep->residual);
+        p.residual = ep->residual;
         p.ldr = ep->ldr;
         p.act = ep->act;
         p.out_f32 = ep->out_f32;
@@ -617,12 +635,13 @@ extern "C" int supir_set_gemm_tile_n(int bn) {
     return SUPIR_OK;
 }
 
-extern "C" int supir_gemm_bf16(const void* A, long long lda, const void* W, long long ldw, void* out, long long ldc,
-                               int M, int N, int K, const supir_epilogue* ep, void* stream) {
-    SUPIR_REQUIRE(A && W && out, "supir_gemm_bf16: null pointer");
-    SUPIR_REQUIRE(M > 0 && N > 0 && K > 0, "supir_gemm_bf16: bad shape M=%d N=%d K=%d", M, N, K);
-    SUPIR_REQUIRE(lda % 8 == 0 && ldw % 8 == 0, "supir_gemm_bf16: lda/ldw must be multiples of 8");
-    SUPIR_REQUIRE(lda >= K && ldw >= K, "supir_gemm_bf16: leading dims smaller than K");
+template <class E>
+static int gemm_impl(const char* who, const void* A, long long lda, const void* W, long long ldw, void* out, long long ldc, int M,
+                     int N, int K, const supir_epilogue* ep, void* stream) {
+    SUPIR_REQUIRE(A && W && out, "%s: null pointer", who);
+    SUPIR_REQUIRE(M > 0 && N > 0 && K > 0, "%s: bad shape M=%d N=%d K=%d", who, M, N, K);
+    SUPIR_REQUIRE(lda % 8 == 0 && ldw % 8 == 0, "%s: lda/ldw must be multiples of 8", who);
+    SUPIR_REQUIRE(lda >= K && ldw >= K, "%s: leading dims smaller than K", who);
     GemmKernelParams p{};
     p.M = M; p.N = N; p.K = K;
     p.num_m_tiles = (M + BM - 1) / BM;
@@ -630,7 +649,7 @@ extern "C" int supir_gemm_bf16(const void* A, long long lda, const void* W, long
     p.conv = 0;
     int rc = fill_epilogue(p, ep, N);
     if (rc) return rc;
-    SUPIR_REQUIRE(ldc >= p.n_out, "supir_gemm_bf16: ldc %lld < output columns %d", ldc, p.n_out);
+    SUPIR_REQUIRE(ldc >= p.n_out, "%s: ldc %lld < output columns %d", who, ldc, p.n_out);
     p.out = out; p.ldc = ldc;
     const int bn = pick_bn(p, g_force_bn);
     CUtensorMap tmA, tmB;
@@ -638,19 +657,20 @@ extern "C" int supir_gemm_bf16(const void* A, long long lda, const void* W, long
         const uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
         const uint64_t str[1] = {(uint64_t)lda};
         const uint32_t box[2] = {BK, BM};
-        rc = make_tmap_bf16(&tmA, A, 2, dims, str, box);
+        rc = make_tmap_16(&tmA, E::kTma, A, 2, dims, str, box);
         if (rc) return rc;
     }
     {
         const uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
         const uint64_t str[1] = {(uint64_t)ldw};
         const uint32_t box[2] = {BK, (uint32_t)bn};
-        rc = make_tmap_bf16(&tmB, W, 2, dims, str, box);
+        rc = make_tmap_16(&tmB, E::kTma, W, 2, dims, str, box);
         if (rc) return rc;
     }
-    return run_gemm(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
+    return run_gemm<E>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
 }
 
+template <class E>
 static int conv_geom_impl(const char* who, const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int Hin, int Win,
                           int Cin, int Cout, const supir_conv_geometry& g, const supir_epilogue* ep, void* stream) {
     SUPIR_REQUIRE(x && Wp && out, "%s: null pointer", who);
@@ -699,30 +719,56 @@ static int conv_geom_impl(const char* who, const void* x, long long ldx, const v
         const uint64_t str[3] = {(uint64_t)ldx, (uint64_t)ldx * Win, (uint64_t)ldx * Win * Hin};
         const uint32_t box[4] = {BK, (uint32_t)(p.TW * g.stride), (uint32_t)(p.TH * g.stride), 1};
         const uint32_t est[4] = {1, (uint32_t)g.stride, (uint32_t)g.stride, 1};
-        rc = make_tmap_bf16_strided(&tmA, x, 4, dims, str, box, est);
+        rc = make_tmap_16_strided(&tmA, E::kTma, x, 4, dims, str, box, est);
         if (rc) return rc;
     }
     {
         const uint64_t dims[2] = {(uint64_t)(ntaps * Cin), (uint64_t)Cout};
         const uint64_t str[1] = {(uint64_t)(ntaps * Cin)};
         const uint32_t box[2] = {BK, (uint32_t)bn};
-        rc = make_tmap_bf16(&tmB, Wp, 2, dims, str, box);
+        rc = make_tmap_16(&tmB, E::kTma, Wp, 2, dims, str, box);
         if (rc) return rc;
     }
-    return run_gemm(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
+    return run_gemm<E>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int supir_gemm_bf16(const void* A, long long lda, const void* W, long long ldw, void* out, long long ldc,
+                               int M, int N, int K, const supir_epilogue* ep, void* stream) {
+    return gemm_impl<Bf16>("supir_gemm_bf16", A, lda, W, ldw, out, ldc, M, N, K, ep, stream);
+}
+
+extern "C" int supir_gemm_f16(const void* A, long long lda, const void* W, long long ldw, void* out, long long ldc,
+                              int M, int N, int K, const supir_epilogue* ep, void* stream) {
+    return gemm_impl<F16>("supir_gemm_f16", A, lda, W, ldw, out, ldc, M, N, K, ep, stream);
 }
 
 extern "C" int supir_conv_geom_bf16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int Hin, int Win,
                                     int Cin, int Cout, const supir_conv_geometry* geom, const supir_epilogue* ep, void* stream) {
     SUPIR_REQUIRE(geom, "supir_conv_geom_bf16: null geometry");
-    return conv_geom_impl("supir_conv_geom_bf16", x, ldx, Wp, out, ldc, B, Hin, Win, Cin, Cout, *geom, ep, stream);
+    return conv_geom_impl<Bf16>("supir_conv_geom_bf16", x, ldx, Wp, out, ldc, B, Hin, Win, Cin, Cout, *geom, ep, stream);
 }
 
-extern "C" int supir_conv3x3_bf16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int H,
-                                  int Wd, int Cin, int Cout, const supir_epilogue* ep, void* stream) {
+extern "C" int supir_conv_geom_f16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int Hin, int Win,
+                                   int Cin, int Cout, const supir_conv_geometry* geom, const supir_epilogue* ep, void* stream) {
+    SUPIR_REQUIRE(geom, "supir_conv_geom_f16: null geometry");
+    return conv_geom_impl<F16>("supir_conv_geom_f16", x, ldx, Wp, out, ldc, B, Hin, Win, Cin, Cout, *geom, ep, stream);
+}
+
+// 3x3, stride 1, pad 1
+static supir_conv_geometry conv3x3_geometry(int H, int Wd) {
     supir_conv_geometry g{};
     g.kh = g.kw = 3; g.stride = 1; g.off_y = g.off_x = -1;
     g.Hout = H; g.Wout = Wd;
     g.out_sy = g.out_sx = 1; g.out_oy = g.out_ox = 0; g.out_H = H; g.out_W = Wd;
-    return conv_geom_impl("supir_conv3x3_bf16", x, ldx, Wp, out, ldc, B, H, Wd, Cin, Cout, g, ep, stream);
+    return g;
+}
+
+extern "C" int supir_conv3x3_bf16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int H,
+                                  int Wd, int Cin, int Cout, const supir_epilogue* ep, void* stream) {
+    return conv_geom_impl<Bf16>("supir_conv3x3_bf16", x, ldx, Wp, out, ldc, B, H, Wd, Cin, Cout, conv3x3_geometry(H, Wd), ep, stream);
+}
+
+extern "C" int supir_conv3x3_f16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int H,
+                                 int Wd, int Cin, int Cout, const supir_epilogue* ep, void* stream) {
+    return conv_geom_impl<F16>("supir_conv3x3_f16", x, ldx, Wp, out, ldc, B, H, Wd, Cin, Cout, conv3x3_geometry(H, Wd), ep, stream);
 }

@@ -1,5 +1,6 @@
 // supir_b200 — K1/K5/K13 of SURVEY.md §2a: GroupNorm(32) [+SiLU], LayerNorm, tiled-VAE cross-tile GroupNorm.
-// All HBM-bound: 128-bit loads/stores on channels-last bf16, fp32 math, fp64 cross-block sums.
+// All HBM-bound: 128-bit loads/stores on channels-last 16-bit data, fp32 math, fp64 cross-block sums. The diffusion-network
+// kernels are templated on the storage type E (common.cuh): Bf16, or F16 for the _f16 entry points.
 //
 // Reference call sites: GroupNorm32 (sgm/modules/diffusionmodules/util.py:258-276, eps 1e-5) in ResBlock
 // (openaimodel.py:260-264,295-308), ZeroSFT/ZeroCrossAttn (SUPIR/modules/SUPIR_v0.py:72,110,128-129);
@@ -18,7 +19,8 @@ int current_device_slot();
 // adds the block partials in block order into sums[b, g, 0:2].
 // workspace layout (doubles): [B*G*2 final sums][B*nblk*G*2 block partials][B tickets (as uint32 in 8-byte slots)]
 // ---------------------------------------------------------------------------------------------
-__global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int C, int G,
+template <class E>
+__global__ void gn_stats_kernel(const typename E::T* __restrict__ x, long long ldx, int HW, int C, int G,
                                 int pixels_per_block, double* __restrict__ ws, int B) {
     extern __shared__ float sm[];  // [2][kp][C]
     __shared__ int is_last;
@@ -36,13 +38,13 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x, long long l
     float s[8], ss[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) s[j] = ss[j] = 0.f;
-    const __nv_bfloat16* base = x + ((long long)b * HW) * ldx + cv * 8;
+    const typename E::T* base = x + ((long long)b * HW) * ldx + cv * 8;
     for (int p = p0 + pl; p < p1; p += kp) {
         const uint4 u = __ldg(reinterpret_cast<const uint4*>(base + (long long)p * ldx));
         const uint32_t w[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
-            const float2 f = unpack_bf16x2(w[t]);
+            const float2 f = E::unpack2(w[t]);
             s[2 * t] += f.x; ss[2 * t] += f.x * f.x;
             s[2 * t + 1] += f.y; ss[2 * t + 1] += f.y * f.y;
         }
@@ -165,9 +167,10 @@ __device__ __forceinline__ void gn_scale_shift(int b, int c0, int C, int G, cons
     }
 }
 
-// y = (x - mean) * rsqrt(var + eps) * gamma + beta [-> SiLU] ; bf16 in, bf16 out, channels-last.
+// y = (x - mean) * rsqrt(var + eps) * gamma + beta [-> SiLU] ; E in, E out, channels-last.
 // block = kp pixel lanes x (C/8) channel vectors; a thread keeps its vector's scale / shift in registers and walks pixels.
-__global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, __nv_bfloat16* __restrict__ y,
+template <class E>
+__global__ void gn_apply_kernel(const typename E::T* __restrict__ x, long long ldx, typename E::T* __restrict__ y,
                                 long long ldy, int HW, int C, int G, const float* __restrict__ mean,
                                 const float* __restrict__ var, const double* __restrict__ sums, double count,
                                 const float* __restrict__ gamma, const float* __restrict__ beta, float eps, int silu,
@@ -181,18 +184,18 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long l
     gn_scale_shift(b, cv * 8, C, G, sums, count, mean, var, gamma, beta, eps, sc, sh);
     const int p0 = blockIdx.x * pixels_per_block;
     const int p1 = min(p0 + pixels_per_block, HW);
-    const __nv_bfloat16* xb = x + ((long long)b * HW) * ldx + cv * 8;
-    __nv_bfloat16* yb = y + ((long long)b * HW) * ldy + cv * 8;
+    const typename E::T* xb = x + ((long long)b * HW) * ldx + cv * 8;
+    typename E::T* yb = y + ((long long)b * HW) * ldy + cv * 8;
     auto one = [&](const uint4 u, long long p) {
         const uint32_t w[4] = {u.x, u.y, u.z, u.w};
         uint32_t o[4];
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
-            const float2 f = unpack_bf16x2(w[t]);
+            const float2 f = E::unpack2(w[t]);
             float a = f.x * sc[2 * t] + sh[2 * t];
             float d = f.y * sc[2 * t + 1] + sh[2 * t + 1];
             if (silu) { a = silu_f(a); d = silu_f(d); }
-            o[t] = pack_bf16x2(a, d);
+            o[t] = E::pack2(a, d);
         }
         __stcs(reinterpret_cast<uint4*>(yb + p * ldy), make_uint4(o[0], o[1], o[2], o[3]));
     };
@@ -212,9 +215,10 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x, long long l
 //   h      : [B, HW, C]  (= cat(h_ori, skip + zero_conv(c)))        gb : [B, HW, 2C] = (gamma | beta) conv outputs
 //   h_raw first C1 channels equal h's; the remaining C - C1 come from `skip_raw` [B, HW, C - C1]
 // ---------------------------------------------------------------------------------------------
-__global__ void sft_apply_kernel(const __nv_bfloat16* __restrict__ h, long long ldh,
-                                 const __nv_bfloat16* __restrict__ skip_raw, long long lds, int C1,
-                                 const __nv_bfloat16* __restrict__ gb, long long ldgb, __nv_bfloat16* __restrict__ out,
+template <class E>
+__global__ void sft_apply_kernel(const typename E::T* __restrict__ h, long long ldh,
+                                 const typename E::T* __restrict__ skip_raw, long long lds, int C1,
+                                 const typename E::T* __restrict__ gb, long long ldgb, typename E::T* __restrict__ out,
                                  long long ldo, int HW, int C, int G, const double* __restrict__ sums, double count,
                                  const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
                                  const float* __restrict__ control_scale, int pixels_per_block) {
@@ -242,13 +246,12 @@ __global__ void sft_apply_kernel(const __nv_bfloat16* __restrict__ h, long long 
         uint32_t o[4];
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
-            const float2 fh = unpack_bf16x2(wh[t]), fg = unpack_bf16x2(wg[t]), fb = unpack_bf16x2(wb[t]),
-                         fr = unpack_bf16x2(wr[t]);
-            // normalised (fp32) * (gamma + 1) + beta, each intermediate rounded like the reference's bf16 tensors
+            const float2 fh = E::unpack2(wh[t]), fg = E::unpack2(wg[t]), fb = E::unpack2(wb[t]), fr = E::unpack2(wr[t]);
+            // normalised (fp32) * (gamma + 1) + beta, each intermediate rounded like the reference's 16-bit tensors
             const float n0 = fh.x * sc[2 * t] + sh[2 * t], n1 = fh.y * sc[2 * t + 1] + sh[2 * t + 1];
-            const float a = n0 * (bf16_round(fg.x + 1.f)) + fb.x;
-            const float d = n1 * (bf16_round(fg.y + 1.f)) + fb.y;
-            o[t] = pack_bf16x2(a * cs + fr.x * (1.f - cs), d * cs + fr.y * (1.f - cs));
+            const float a = n0 * (E::round(fg.x + 1.f)) + fb.x;
+            const float d = n1 * (E::round(fg.y + 1.f)) + fb.y;
+            o[t] = E::pack2(a * cs + fr.x * (1.f - cs), d * cs + fr.y * (1.f - cs));
         }
         __stcs(reinterpret_cast<uint4*>(out + row * ldo + c0), make_uint4(o[0], o[1], o[2], o[3]));
     };
@@ -260,8 +263,8 @@ __global__ void sft_apply_kernel(const __nv_bfloat16* __restrict__ h, long long 
 // ---------------------------------------------------------------------------------------------
 // LayerNorm over the last dim (C <= 2048, C % 8 == 0): one warp per row, row kept in registers.
 // ---------------------------------------------------------------------------------------------
-template <int MAXV>  // max 16-byte vectors per lane
-__global__ void layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, __nv_bfloat16* __restrict__ y,
+template <int MAXV, class E>  // max 16-byte vectors per lane
+__global__ void layernorm_kernel(const typename E::T* __restrict__ x, long long ldx, typename E::T* __restrict__ y,
                                  long long ldy, long long rows, int C, const float* __restrict__ gamma,
                                  const float* __restrict__ beta, float eps, float2* __restrict__ stats) {
     const int lane = threadIdx.x & 31;
@@ -287,7 +290,7 @@ __global__ void layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long 
                 const uint32_t w[4] = {nxt[i].x, nxt[i].y, nxt[i].z, nxt[i].w};
 #pragma unroll
                 for (int t = 0; t < 4; ++t) {
-                    const float2 f = unpack_bf16x2(w[t]);
+                    const float2 f = E::unpack2(w[t]);
                     v[i][2 * t] = f.x; v[i][2 * t + 1] = f.y;
                     s += f.x + f.y;
                 }
@@ -329,8 +332,8 @@ __global__ void layernorm_kernel(const __nv_bfloat16* __restrict__ x, long long 
                 uint32_t o[4];
 #pragma unroll
                 for (int t = 0; t < 4; ++t)
-                    o[t] = pack_bf16x2((v[i][2 * t] - mean) * rstd * gg[2 * t] + bb[2 * t],
-                                       (v[i][2 * t + 1] - mean) * rstd * gg[2 * t + 1] + bb[2 * t + 1]);
+                    o[t] = E::pack2((v[i][2 * t] - mean) * rstd * gg[2 * t] + bb[2 * t],
+                                    (v[i][2 * t + 1] - mean) * rstd * gg[2 * t + 1] + bb[2 * t + 1]);
                 __stcs(reinterpret_cast<uint4*>(y + row * ldy + vi * 8), make_uint4(o[0], o[1], o[2], o[3]));
             }
         }
@@ -438,28 +441,39 @@ extern "C" long long supir_groupnorm_stats_workspace(int B, int HW, int C, int g
     return (long long)B * groups * 2 + (long long)B * bx * groups * 2 + B;
 }
 
-extern "C" int supir_groupnorm_stats(const void* x, long long ldx, int B, int HW, int C, int groups, double* ws,
-                                     long long ws_doubles, void* stream) {
-    SUPIR_REQUIRE(x && ws, "supir_groupnorm_stats: null pointer");
-    SUPIR_REQUIRE(C % 8 == 0 && C % groups == 0 && ldx % 8 == 0 && C <= 8192, "supir_groupnorm_stats: bad C=%d", C);
+template <class E>
+static int groupnorm_stats_impl(const char* who, const void* x, long long ldx, int B, int HW, int C, int groups, double* ws,
+                                long long ws_doubles, void* stream) {
+    SUPIR_REQUIRE(x && ws, "%s: null pointer", who);
+    SUPIR_REQUIRE(C % 8 == 0 && C % groups == 0 && ldx % 8 == 0 && C <= 8192, "%s: bad C=%d", who, C);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     int threads, ppb, bx;
     gn_launch_shape(HW, C, threads, ppb, bx);
     const long long need = (long long)B * groups * 2 + (long long)B * bx * groups * 2 + B;
-    SUPIR_REQUIRE(ws_doubles >= need, "supir_groupnorm_stats: workspace of %lld doubles < %lld required", ws_doubles, need);
+    SUPIR_REQUIRE(ws_doubles >= need, "%s: workspace of %lld doubles < %lld required", who, ws_doubles, need);
     SUPIR_CHECK_CUDA(cudaMemsetAsync(ws + need - B, 0, sizeof(double) * B, st));   // tickets
     const int kp = threads / (C >> 3);
     const size_t smem = (size_t)2 * kp * C * sizeof(float);
     static size_t max_set_dev[64] = {};
     size_t& max_set = max_set_dev[current_device_slot()];
     if (smem > 48 * 1024 && smem > max_set) {
-        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(gn_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SUPIR_CHECK_CUDA(cudaFuncSetAttribute(gn_stats_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         max_set = smem;
     }
-    gn_stats_kernel<<<dim3(bx, B), threads, smem, st>>>(reinterpret_cast<const __nv_bfloat16*>(x), ldx, HW, C, groups, ppb, ws, B);
+    gn_stats_kernel<E><<<dim3(bx, B), threads, smem, st>>>(reinterpret_cast<const typename E::T*>(x), ldx, HW, C, groups, ppb, ws, B);
     count_launch();
     SUPIR_CHECK_CUDA(cudaGetLastError());
     return SUPIR_OK;
+}
+
+extern "C" int supir_groupnorm_stats(const void* x, long long ldx, int B, int HW, int C, int groups, double* ws,
+                                     long long ws_doubles, void* stream) {
+    return groupnorm_stats_impl<Bf16>("supir_groupnorm_stats", x, ldx, B, HW, C, groups, ws, ws_doubles, stream);
+}
+
+extern "C" int supir_groupnorm_stats_f16(const void* x, long long ldx, int B, int HW, int C, int groups, double* ws,
+                                         long long ws_doubles, void* stream) {
+    return groupnorm_stats_impl<F16>("supir_groupnorm_stats_f16", x, ldx, B, HW, C, groups, ws, ws_doubles, stream);
 }
 
 extern "C" int supir_groupnorm_finalize(const double* sums, int n, double count, float* mean, float* var, void* stream) {
@@ -480,12 +494,12 @@ extern "C" int supir_groupnorm_merge_tiles(const float* tile_mean, const float* 
     return SUPIR_OK;
 }
 
-extern "C" int supir_groupnorm_apply(const void* x, long long ldx, void* y, long long ldy, int B, int HW, int C,
-                                     int groups, const double* sums, const float* mean, const float* var,
-                                     const float* gamma, const float* beta, float eps, int silu, void* stream) {
-    SUPIR_REQUIRE(x && y && (sums || (mean && var)), "supir_groupnorm_apply: null pointer");
-    SUPIR_REQUIRE(C % 8 == 0 && C % groups == 0 && ldx % 8 == 0 && ldy % 8 == 0 && C <= 8192,
-                  "supir_groupnorm_apply: bad C=%d", C);
+template <class E>
+static int groupnorm_apply_impl(const char* who, const void* x, long long ldx, void* y, long long ldy, int B, int HW, int C,
+                                int groups, const double* sums, const float* mean, const float* var, const float* gamma,
+                                const float* beta, float eps, int silu, void* stream) {
+    SUPIR_REQUIRE(x && y && (sums || (mean && var)), "%s: null pointer", who);
+    SUPIR_REQUIRE(C % 8 == 0 && C % groups == 0 && ldx % 8 == 0 && ldy % 8 == 0 && C <= 8192, "%s: bad C=%d", who, C);
     const int cvc = C >> 3;
     int kp = 512 / cvc;
     if (kp < 1) kp = 1;
@@ -493,9 +507,47 @@ extern "C" int supir_groupnorm_apply(const void* x, long long ldx, void* y, long
     int ppb = kp * 32;              // 32 pixels per thread amortise the per-thread scale / shift set-up
     if (ppb > HW) ppb = (HW + kp - 1) / kp * kp;
     const int bx = (HW + ppb - 1) / ppb;
-    gn_apply_kernel<<<dim3(bx, B), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<__nv_bfloat16*>(y), ldy, HW, C, groups, mean,
+    gn_apply_kernel<E><<<dim3(bx, B), threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<const typename E::T*>(x), ldx, reinterpret_cast<typename E::T*>(y), ldy, HW, C, groups, mean,
         var, sums, (double)HW * (C / groups), gamma, beta, eps, silu, ppb);
+    count_launch();
+    SUPIR_CHECK_CUDA(cudaGetLastError());
+    return SUPIR_OK;
+}
+
+extern "C" int supir_groupnorm_apply(const void* x, long long ldx, void* y, long long ldy, int B, int HW, int C,
+                                     int groups, const double* sums, const float* mean, const float* var,
+                                     const float* gamma, const float* beta, float eps, int silu, void* stream) {
+    return groupnorm_apply_impl<Bf16>("supir_groupnorm_apply", x, ldx, y, ldy, B, HW, C, groups, sums, mean, var, gamma, beta,
+                                      eps, silu, stream);
+}
+
+extern "C" int supir_groupnorm_apply_f16(const void* x, long long ldx, void* y, long long ldy, int B, int HW, int C,
+                                         int groups, const double* sums, const float* mean, const float* var,
+                                         const float* gamma, const float* beta, float eps, int silu, void* stream) {
+    return groupnorm_apply_impl<F16>("supir_groupnorm_apply_f16", x, ldx, y, ldy, B, HW, C, groups, sums, mean, var, gamma, beta,
+                                     eps, silu, stream);
+}
+
+template <class E>
+static int zerosft_apply_impl(const char* who, const void* h, long long ldh, const void* skip_raw, long long lds, int C1,
+                              const void* gamma_beta, long long ldgb, void* out, long long ldo, int B, int HW, int C, int groups,
+                              const double* sums, const float* gn_weight, const float* gn_bias, float eps,
+                              const float* control_scale, void* stream) {
+    SUPIR_REQUIRE(h && gamma_beta && out && sums && gn_weight && gn_bias && control_scale, "%s: null pointer", who);
+    SUPIR_REQUIRE(C % 8 == 0 && C1 % 8 == 0 && C % groups == 0 && (C1 == C || skip_raw), "%s: bad channels", who);
+    SUPIR_REQUIRE(C <= 8192, "%s: C=%d too large", who, C);
+    const int cvc = C >> 3;
+    int kp = 512 / cvc;
+    if (kp < 1) kp = 1;
+    int ppb = kp * 16;
+    if (ppb > HW) ppb = (HW + kp - 1) / kp * kp;
+    const int bx = (HW + ppb - 1) / ppb;
+    using T = typename E::T;
+    sft_apply_kernel<E><<<dim3(bx, B), kp * cvc, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        reinterpret_cast<const T*>(h), ldh, reinterpret_cast<const T*>(skip_raw), lds, C1,
+        reinterpret_cast<const T*>(gamma_beta), ldgb, reinterpret_cast<T*>(out), ldo, HW, C,
+        groups, sums, (double)HW * (C / groups), gn_weight, gn_bias, eps, control_scale, ppb);
     count_launch();
     SUPIR_CHECK_CUDA(cudaGetLastError());
     return SUPIR_OK;
@@ -505,24 +557,19 @@ extern "C" int supir_zerosft_apply(const void* h, long long ldh, const void* ski
                                    const void* gamma_beta, long long ldgb, void* out, long long ldo, int B, int HW,
                                    int C, int groups, const double* sums, const float* gn_weight, const float* gn_bias,
                                    float eps, const float* control_scale, void* stream) {
-    SUPIR_REQUIRE(h && gamma_beta && out && sums && gn_weight && gn_bias && control_scale, "supir_zerosft_apply: null pointer");
-    SUPIR_REQUIRE(C % 8 == 0 && C1 % 8 == 0 && C % groups == 0 && (C1 == C || skip_raw), "supir_zerosft_apply: bad channels");
-    SUPIR_REQUIRE(C <= 8192, "supir_zerosft_apply: C=%d too large", C);
-    const int cvc = C >> 3;
-    int kp = 512 / cvc;
-    if (kp < 1) kp = 1;
-    int ppb = kp * 16;
-    if (ppb > HW) ppb = (HW + kp - 1) / kp * kp;
-    const int bx = (HW + ppb - 1) / ppb;
-    sft_apply_kernel<<<dim3(bx, B), kp * cvc, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<const __nv_bfloat16*>(h), ldh, reinterpret_cast<const __nv_bfloat16*>(skip_raw), lds, C1,
-        reinterpret_cast<const __nv_bfloat16*>(gamma_beta), ldgb, reinterpret_cast<__nv_bfloat16*>(out), ldo, HW, C,
-        groups, sums, (double)HW * (C / groups), gn_weight, gn_bias, eps, control_scale, ppb);
-    count_launch();
-    SUPIR_CHECK_CUDA(cudaGetLastError());
-    return SUPIR_OK;
+    return zerosft_apply_impl<Bf16>("supir_zerosft_apply", h, ldh, skip_raw, lds, C1, gamma_beta, ldgb, out, ldo, B, HW, C, groups,
+                                    sums, gn_weight, gn_bias, eps, control_scale, stream);
 }
 
+extern "C" int supir_zerosft_apply_f16(const void* h, long long ldh, const void* skip_raw, long long lds, int C1,
+                                       const void* gamma_beta, long long ldgb, void* out, long long ldo, int B, int HW,
+                                       int C, int groups, const double* sums, const float* gn_weight, const float* gn_bias,
+                                       float eps, const float* control_scale, void* stream) {
+    return zerosft_apply_impl<F16>("supir_zerosft_apply_f16", h, ldh, skip_raw, lds, C1, gamma_beta, ldgb, out, ldo, B, HW, C, groups,
+                                   sums, gn_weight, gn_bias, eps, control_scale, stream);
+}
+
+template <class E>
 static int launch_layernorm(const void* x, long long ldx, void* y, long long ldy, long long rows, int C, const float* gamma,
                             const float* beta, float eps, float2* stats, void* stream);
 
@@ -530,16 +577,31 @@ extern "C" int supir_layernorm_stats(const void* x, long long ldx, long long row
     SUPIR_REQUIRE(x && stats && rows > 0, "supir_layernorm_stats: bad args");
     SUPIR_REQUIRE(C % 8 == 0 && C <= 2048 && ldx % 8 == 0, "supir_layernorm_stats: unsupported C=%d", C);
     SUPIR_REQUIRE((reinterpret_cast<uintptr_t>(stats) & 7) == 0, "supir_layernorm_stats: stats must be 8-byte aligned");
-    return launch_layernorm(x, ldx, nullptr, 0, rows, C, nullptr, nullptr, eps, reinterpret_cast<float2*>(stats), stream);
+    return launch_layernorm<Bf16>(x, ldx, nullptr, 0, rows, C, nullptr, nullptr, eps, reinterpret_cast<float2*>(stats), stream);
+}
+
+extern "C" int supir_layernorm_stats_f16(const void* x, long long ldx, long long rows, int C, float eps, float* stats, void* stream) {
+    SUPIR_REQUIRE(x && stats && rows > 0, "supir_layernorm_stats_f16: bad args");
+    SUPIR_REQUIRE(C % 8 == 0 && C <= 2048 && ldx % 8 == 0, "supir_layernorm_stats_f16: unsupported C=%d", C);
+    SUPIR_REQUIRE((reinterpret_cast<uintptr_t>(stats) & 7) == 0, "supir_layernorm_stats_f16: stats must be 8-byte aligned");
+    return launch_layernorm<F16>(x, ldx, nullptr, 0, rows, C, nullptr, nullptr, eps, reinterpret_cast<float2*>(stats), stream);
 }
 
 extern "C" int supir_layernorm_bf16(const void* x, long long ldx, void* y, long long ldy, long long rows, int C,
                                     const float* gamma, const float* beta, float eps, void* stream) {
     SUPIR_REQUIRE(x && y && gamma && beta, "supir_layernorm_bf16: null pointer");
     SUPIR_REQUIRE(C % 8 == 0 && C <= 2048 && ldx % 8 == 0 && ldy % 8 == 0, "supir_layernorm_bf16: unsupported C=%d", C);
-    return launch_layernorm(x, ldx, y, ldy, rows, C, gamma, beta, eps, nullptr, stream);
+    return launch_layernorm<Bf16>(x, ldx, y, ldy, rows, C, gamma, beta, eps, nullptr, stream);
 }
 
+extern "C" int supir_layernorm_f16(const void* x, long long ldx, void* y, long long ldy, long long rows, int C,
+                                   const float* gamma, const float* beta, float eps, void* stream) {
+    SUPIR_REQUIRE(x && y && gamma && beta, "supir_layernorm_f16: null pointer");
+    SUPIR_REQUIRE(C % 8 == 0 && C <= 2048 && ldx % 8 == 0 && ldy % 8 == 0, "supir_layernorm_f16: unsupported C=%d", C);
+    return launch_layernorm<F16>(x, ldx, y, ldy, rows, C, gamma, beta, eps, nullptr, stream);
+}
+
+template <class E>
 static int launch_layernorm(const void* x, long long ldx, void* y, long long ldy, long long rows, int C, const float* gamma,
                             const float* beta, float eps, float2* stats, void* stream) {
     const int warps = 8;
@@ -547,15 +609,15 @@ static int launch_layernorm(const void* x, long long ldx, void* y, long long ldy
     const long long cap = (long long)device_sm_count() * 16;       // a few resident waves; warps then loop over rows
     if (blocks > cap) blocks = cap;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    const __nv_bfloat16* xp = reinterpret_cast<const __nv_bfloat16*>(x);
-    __nv_bfloat16* yp = reinterpret_cast<__nv_bfloat16*>(y);
+    const typename E::T* xp = reinterpret_cast<const typename E::T*>(x);
+    typename E::T* yp = reinterpret_cast<typename E::T*>(y);
     const int nv = C >> 3;
     if (nv <= 96)
-        layernorm_kernel<3><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats);
+        layernorm_kernel<3, E><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats);
     else if (nv <= 160)
-        layernorm_kernel<5><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats);
+        layernorm_kernel<5, E><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats);
     else
-        layernorm_kernel<8><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats);
+        layernorm_kernel<8, E><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats);
     count_launch();
     SUPIR_CHECK_CUDA(cudaGetLastError());
     return SUPIR_OK;

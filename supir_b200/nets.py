@@ -3,9 +3,10 @@
 Same constructor parameters and state_dict key names as the reference classes (SUPIR/modules/SUPIR_v0.py:155-666,
 sgm/modules/diffusionmodules/openaimodel.py:506-961, sgm/modules/attention.py:196-635) so the reference's YAML configs and
 checkpoints load unchanged — but the torch modules below only OWN parameters. Nothing here runs a torch op on the hot
-path: `pack()` converts the weights once into the kernel layouts (bf16, K-major, fused QKV / KV / GEGLU / gamma|beta
-matrices, fp32 biases) and `run()` issues hand-written sm_90a kernels through the C ABI (supir_b200/ops.py) on
-channels-last bf16 activations. Options the SUPIR configs never use raise NotImplementedError.
+path: `pack(dtype)` converts the weights once into the kernel layouts (bf16 or fp16, K-major, fused QKV / KV / GEGLU /
+gamma|beta matrices, fp32 biases) and `run()` issues hand-written sm_90a kernels through the C ABI (supir_b200/ops.py) on
+channels-last activations of that dtype (torch.autocast(bfloat16) or autocast(float16) numerics). Options the SUPIR configs
+never use raise NotImplementedError.
 """
 import os
 
@@ -24,7 +25,7 @@ GN_EPS_ATTN = 1e-6   # attention.Normalize (sgm/modules/attention.py:122-125)
 
 
 class Act:
-    """Channels-last activation: t is a bf16 matrix [B*H*W, C] (row stride = leading dimension)."""
+    """Channels-last activation: t is a bf16 or fp16 matrix [B*H*W, C] (row stride = leading dimension)."""
     __slots__ = ("t", "B", "H", "W")
 
     def __init__(self, t, B, H, W):
@@ -44,19 +45,21 @@ class Act:
 
 
 class Ctx:
-    """Per-call execution context: scratch pool, conditioning tensors, device scalars."""
+    """Per-call execution context: scratch pool, conditioning tensors, device scalars, compute dtype (bf16 or fp16: the
+    dtype the networks were packed in, and of every activation `new` allocates)."""
 
-    def __init__(self, pool, B):
+    def __init__(self, pool, B, dtype=BF16):
         self.pool = pool
         self.B = B
+        self.dtype = dtype
         self.emb_all = None        # fp32 [B, sum(Cout of all ResBlocks)]
-        self.ctx_kv = None         # bf16 [B*Lctx, sum(2*inner)] context K|V projections of every cross-attention
+        self.ctx_kv = None         # [B*Lctx, sum(2*inner)] context K|V projections of every cross-attention (compute dtype)
         self.kv_owned = True       # False: ctx_kv belongs to the caller (projected outside the per-step graph)
         self.Lctx = 0
         self.control_scale = None  # fp32 device scalar
 
-    def new(self, rows, cols, dtype=BF16):
-        return self.pool.get((rows, cols), dtype)
+    def new(self, rows, cols, dtype=None):
+        return self.pool.get((rows, cols), dtype or self.dtype)
 
     def free(self, *ts):
         self.pool.put(*[t.t if isinstance(t, Act) else t for t in ts])
@@ -66,18 +69,24 @@ def _f32(t):
     return t.detach().to(torch.float32).contiguous()
 
 
-def _bf(t):
-    return t.detach().to(BF16).contiguous()
+def _bf(t, dtype=BF16):
+    """Weights as the 16-bit GEMM operand (`dtype`: bf16, or fp16 for the fp16 compute mode)."""
+    return t.detach().to(dtype).contiguous()
+
+
+def _bias_values(t, dtype):
+    """autocast hands the bias to the 16-bit GEMM; keep those values (rounded to `dtype`, bf16 or fp16), stored as fp32 for
+    the epilogue."""
+    return None if t is None else t.detach().to(dtype).to(torch.float32).contiguous()
 
 
 def _bias_bf16_values(t):
-    """autocast hands the bias to the bf16 GEMM; keep those values, stored as fp32 for the epilogue."""
-    return None if t is None else t.detach().to(BF16).to(torch.float32).contiguous()
+    return _bias_values(t, BF16)
 
 
-def pack_conv3x3(w):
+def pack_conv3x3(w, dtype=BF16):
     """[Cout, Cin, 3, 3] -> [Cout, 9*Cin] with k = (kh*3 + kw)*Cin + cin (what supir_conv3x3_bf16 / im2col expect)."""
-    return _bf(w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1))
+    return _bf(w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], -1), dtype)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -114,9 +123,9 @@ class TimestepEmbedSequential(nn.Sequential):
 class ConvIn(nn.Conv2d):
     """4 -> model_channels 3x3 conv fed with fp32 NCHW (input_blocks.0.0, input_hint_block.0)."""
 
-    def pack(self):
-        self._w, self._b = self.weight.detach().to(BF16).to(torch.float32).contiguous(), _bias_bf16_values(self.bias)
-        self._wp = ops.pack_small_cin_weight(self.weight)
+    def pack(self, dtype=BF16):
+        self._w, self._b = self.weight.detach().to(dtype).to(torch.float32).contiguous(), _bias_values(self.bias, dtype)
+        self._wp = ops.pack_small_cin_weight(self.weight, dtype)
 
     def run_nchw(self, ctx, x_nchw, residual=None):
         B, _, H, W = x_nchw.shape
@@ -142,13 +151,13 @@ class ResBlock(nn.Module):
         self.skip_connection = nn.Identity() if self.out_channels == channels else nn.Conv2d(channels, self.out_channels, 1)
         self.emb_offset = None
 
-    def pack(self):
+    def pack(self, dtype=BF16):
         pack_norm(self.in_layers[0]), pack_norm(self.out_layers[0])
-        self._w1, self._b1 = pack_conv3x3(self.in_layers[2].weight), _bias_bf16_values(self.in_layers[2].bias)
-        self._w2, self._b2 = pack_conv3x3(self.out_layers[3].weight), _bias_bf16_values(self.out_layers[3].bias)
+        self._w1, self._b1 = pack_conv3x3(self.in_layers[2].weight, dtype), _bias_values(self.in_layers[2].bias, dtype)
+        self._w2, self._b2 = pack_conv3x3(self.out_layers[3].weight, dtype), _bias_values(self.out_layers[3].bias, dtype)
         if isinstance(self.skip_connection, nn.Conv2d):
-            self._ws = _bf(self.skip_connection.weight.reshape(self.out_channels, self.channels))
-            self._bs = _bias_bf16_values(self.skip_connection.bias)
+            self._ws = _bf(self.skip_connection.weight.reshape(self.out_channels, self.channels), dtype)
+            self._bs = _bias_values(self.skip_connection.bias, dtype)
 
     def run(self, ctx, x: Act):
         n1 = group_norm(ctx, x, self.in_layers[0], silu=True)
@@ -182,8 +191,8 @@ class Downsample(nn.Module):
         self.channels, self.out_channels = channels, out_channels or channels
         self.op = nn.Conv2d(channels, self.out_channels, 3, stride=2, padding=1)
 
-    def pack(self):
-        self._w, self._b = pack_conv3x3(self.op.weight), _bias_bf16_values(self.op.bias)
+    def pack(self, dtype=BF16):
+        self._w, self._b = pack_conv3x3(self.op.weight, dtype), _bias_values(self.op.bias, dtype)
 
     def run(self, ctx, x: Act):
         Ho, Wo = (x.H + 2 - 3) // 2 + 1, (x.W + 2 - 3) // 2 + 1
@@ -208,12 +217,12 @@ class Upsample(nn.Module):
         self.channels, self.out_channels = channels, out_channels or channels
         self.conv = nn.Conv2d(channels, self.out_channels, 3, padding=1)
 
-    def pack(self):
-        self._b = _bias_bf16_values(self.conv.bias)
+    def pack(self, dtype=BF16):
+        self._b = _bias_values(self.conv.bias, dtype)
         if ops.CONV_GEOM:
-            self._wfold = ops.fold_upsample_weights(self.conv.weight)
+            self._wfold = ops.fold_upsample_weights(self.conv.weight, dtype)
         else:
-            self._w = pack_conv3x3(self.conv.weight)
+            self._w = pack_conv3x3(self.conv.weight, dtype)
 
     def run(self, ctx, x: Act):
         out = ctx.new(4 * x.rows, self.out_channels)
@@ -246,20 +255,20 @@ class CrossAttention(nn.Module):
 
     _ln = None      # (gamma, beta) of the LayerNorm in front of the query projection, set by BasicTransformerBlock.pack
 
-    def pack(self):
+    def pack(self, dtype=BF16):
         if self.is_self:
             wqkv = torch.cat([self.to_q.weight, self.to_k.weight, self.to_v.weight], 0)
             if self._ln is not None:
-                self._wqkv, self._c1, self._bq = ops.fold_layernorm(wqkv, None, *self._ln)
+                self._wqkv, self._c1, self._bq = ops.fold_layernorm(wqkv, None, *self._ln, dtype=dtype)
             else:
-                self._wqkv, self._c1, self._bq = _bf(wqkv), None, None
+                self._wqkv, self._c1, self._bq = _bf(wqkv, dtype), None, None
         else:
             if self._ln is not None:
-                self._wq, self._c1, self._bq = ops.fold_layernorm(self.to_q.weight, None, *self._ln)
+                self._wq, self._c1, self._bq = ops.fold_layernorm(self.to_q.weight, None, *self._ln, dtype=dtype)
             else:
-                self._wq, self._c1, self._bq = _bf(self.to_q.weight), None, None
-            self._wkv = _bf(torch.cat([self.to_k.weight, self.to_v.weight], 0))
-        self._wo, self._bo = _bf(self.to_out[0].weight), _bias_bf16_values(self.to_out[0].bias)
+                self._wq, self._c1, self._bq = _bf(self.to_q.weight, dtype), None, None
+            self._wkv = _bf(torch.cat([self.to_k.weight, self.to_v.weight], 0), dtype)
+        self._wo, self._bo = _bf(self.to_out[0].weight, dtype), _bias_values(self.to_out[0].bias, dtype)
 
     def _ln_args(self, stats):
         """gemm() keywords of the query-side projection: folded LayerNorm when this module was packed with one."""
@@ -311,15 +320,15 @@ class FeedForward(nn.Module):
         self.inner = inner
         self.net = nn.Sequential(GEGLU(dim, inner), nn.Dropout(dropout), nn.Linear(inner, dim))
 
-    def pack(self):
+    def pack(self, dtype=BF16):
         w, b = self.net[0].proj.weight.detach(), self.net[0].proj.bias.detach()
         inner = self.inner
         assert inner % 16 == 0
         # interleave value / gate rows in groups of 16 so that each 32-column accumulator chunk holds both halves
         idx = torch.arange(inner, device=w.device).view(-1, 16)
         perm = torch.cat([idx, idx + inner], dim=1).reshape(-1)
-        self._w1, self._b1 = _bf(w[perm]), _bias_bf16_values(b[perm])
-        self._w2, self._b2 = _bf(self.net[2].weight), _bias_bf16_values(self.net[2].bias)
+        self._w1, self._b1 = _bf(w[perm], dtype), _bias_values(b[perm], dtype)
+        self._w2, self._b2 = _bf(self.net[2].weight, dtype), _bias_values(self.net[2].bias, dtype)
 
     def run(self, ctx, xn, x_res):
         g = ctx.new(xn.shape[0], self.inner)
@@ -342,7 +351,7 @@ class BasicTransformerBlock(nn.Module):
         self.attn2 = CrossAttention(query_dim=dim, context_dim=context_dim, heads=n_heads, dim_head=d_head, dropout=dropout)
         self.norm1, self.norm2, self.norm3 = nn.LayerNorm(dim), nn.LayerNorm(dim), nn.LayerNorm(dim)
 
-    def pack(self):
+    def pack(self, dtype=BF16):
         for n in (self.norm1, self.norm2, self.norm3):
             pack_norm(n)
         # norm1 -> QKV and norm2 -> to_q are folded into those GEMMs (runs before the children's pack(): modules() yields
@@ -394,10 +403,10 @@ class SpatialTransformer(nn.Module):
             [BasicTransformerBlock(inner, n_heads, d_head, dropout=dropout, context_dim=context_dim) for _ in range(depth)])
         self.proj_out = nn.Linear(inner, in_channels)
 
-    def pack(self):
+    def pack(self, dtype=BF16):
         pack_norm(self.norm)
-        self._wi, self._bi = _bf(self.proj_in.weight), _bias_bf16_values(self.proj_in.bias)
-        self._wo, self._bo = _bf(self.proj_out.weight), _bias_bf16_values(self.proj_out.bias)
+        self._wi, self._bi = _bf(self.proj_in.weight, dtype), _bias_values(self.proj_in.bias, dtype)
+        self._wo, self._bo = _bf(self.proj_out.weight, dtype), _bias_values(self.proj_out.bias, dtype)
 
     def run(self, ctx, x: Act):
         n = group_norm(ctx, x, self.norm, silu=False)
@@ -429,13 +438,14 @@ class ZeroSFT(nn.Module):
         self.pre_concat = concat_channels != 0
         self.mask = mask
 
-    def pack(self):
+    def pack(self, dtype=BF16):
         pack_norm(self.param_free_norm)
-        self._ws, self._bs = pack_conv3x3(self.mlp_shared[0].weight), _bias_bf16_values(self.mlp_shared[0].bias)
-        self._wgb = torch.cat([pack_conv3x3(self.zero_mul.weight), pack_conv3x3(self.zero_add.weight)], 0).contiguous()
-        self._bgb = torch.cat([_bias_bf16_values(self.zero_mul.bias), _bias_bf16_values(self.zero_add.bias)], 0).contiguous()
-        self._wz = _bf(self.zero_conv.weight.reshape(self.norm_nc, self.label_nc))
-        self._bz = _bias_bf16_values(self.zero_conv.bias)
+        self._ws, self._bs = pack_conv3x3(self.mlp_shared[0].weight, dtype), _bias_values(self.mlp_shared[0].bias, dtype)
+        self._wgb = torch.cat([pack_conv3x3(self.zero_mul.weight, dtype), pack_conv3x3(self.zero_add.weight, dtype)], 0).contiguous()
+        self._bgb = torch.cat([_bias_values(self.zero_mul.bias, dtype), _bias_values(self.zero_add.bias, dtype)],
+                              0).contiguous()
+        self._wz = _bf(self.zero_conv.weight.reshape(self.norm_nc, self.label_nc), dtype)
+        self._bz = _bias_values(self.zero_conv.bias, dtype)
 
     def run(self, ctx, c: Act, h: Act, h_ori: Act = None):
         if h_ori is not None and not self.pre_concat:
@@ -471,7 +481,7 @@ class ZeroCrossAttn(nn.Module):
         self.norm2 = GroupNorm32(32, context_dim)
         self.mask = mask
 
-    def pack(self):
+    def pack(self, dtype=BF16):
         pack_norm(self.norm1), pack_norm(self.norm2)
 
     def run(self, ctx, context: Act, x: Act):
@@ -546,8 +556,11 @@ class _UNetBase(nn.Module):
         return chans, ch, ds, ted, transformer_depth, st
 
     # ---- packing -----------------------------------------------------------------------------------------------------
-    def pack(self):
-        """Convert parameters into kernel layouts (call again after load_state_dict / .to())."""
+    def pack(self, dtype=BF16):
+        """Convert parameters into kernel layouts (call again after load_state_dict / .to()). `dtype` is the compute dtype:
+        torch.bfloat16, or torch.float16 for the fp16 mode (every 16-bit weight, bias value and activation in fp16)."""
+        if dtype not in (BF16, ops.F16):
+            raise ValueError(f"compute dtype {dtype} is not supported (bfloat16 or float16)")
         res, xattn = [], []
         for m in self.modules():
             if isinstance(m, ResBlock):
@@ -558,8 +571,8 @@ class _UNetBase(nn.Module):
         for r in res:
             r.emb_offset = off
             off += r.out_channels
-        self._emb_w = _bf(torch.cat([r.emb_layers[1].weight for r in res], 0))
-        self._emb_b = torch.cat([_bias_bf16_values(r.emb_layers[1].bias) for r in res], 0).contiguous()
+        self._emb_w = _bf(torch.cat([r.emb_layers[1].weight for r in res], 0), dtype)
+        self._emb_b = torch.cat([_bias_values(r.emb_layers[1].bias, dtype) for r in res], 0).contiguous()
         off = 0
         for a in xattn:
             a.kv_offset = off
@@ -567,22 +580,26 @@ class _UNetBase(nn.Module):
         self._ctx_kv_cols = off
         for m in self.modules():
             if m is not self and hasattr(m, "pack") and not isinstance(m, _UNetBase):
-                m.pack()
+                m.pack(dtype)
         # text K|V projection of every cross-attention as ONE weight matrix [sum(2*inner), context_dim]
         self._ctx_w = torch.cat([a._wkv for a in xattn], 0).contiguous()
         te, le = self.time_embed, self.label_emb[0]
-        self._te = (_bf(te[0].weight), _bias_bf16_values(te[0].bias), _bf(te[2].weight), _bias_bf16_values(te[2].bias))
-        self._le = (_bf(le[0].weight), _bias_bf16_values(le[0].bias), _bf(le[2].weight), _bias_bf16_values(le[2].bias))
+        self._te = (_bf(te[0].weight, dtype), _bias_values(te[0].bias, dtype), _bf(te[2].weight, dtype),
+                    _bias_values(te[2].bias, dtype))
+        self._le = (_bf(le[0].weight, dtype), _bias_values(le[0].bias, dtype), _bf(le[2].weight, dtype),
+                    _bias_values(le[2].bias, dtype))
         self._packed_device = self._emb_w.device
+        self._packed_dtype = dtype
         return self
 
-    def project_context(self, context_bf16, out):
+    def project_context(self, context_16, out):
         """Text K|V of EVERY cross-attention of this network as one GEMM: out[B*Lctx, sum 2*inner] (attention.py:248-251).
+        The context and `out` are in the packed compute dtype.
         The context is constant over the sampler steps, so ControlWrapper runs this outside the per-step CUDA graph and
         only when the context changes."""
-        return ops.gemm(context_bf16, self._ctx_w, out)
+        return ops.gemm(context_16, self._ctx_w, out)
 
-    def _prepare_ctx(self, ctx, t_f32, context_bf16, B, Lctx, y_f32, ctx_kv=None):
+    def _prepare_ctx(self, ctx, t_f32, context_16, B, Lctx, y_f32, ctx_kv=None):
         """K8: timestep + label embedding MLPs and every ResBlock's emb projection; text K|V for all cross-attentions
         (`ctx_kv`: already projected by project_context)."""
         p = ctx.pool
@@ -597,8 +614,8 @@ class _UNetBase(nn.Module):
         ops.linear_small_m(h2, self._le[2], self._le[3], emb, add=e_t, silu_out=2)
         ctx.emb_all = p.get((B, self._emb_w.shape[0]), torch.float32)
         if B > 16:      # every ResBlock's emb projection at once: [B, 1280] x [sum Cout, 1280]^T — a tensor-core GEMM beyond a few rows
-            emb_bf = p.get((B, emb.shape[1]))
-            ops.f32_to_bf16(emb, emb_bf)
+            emb_bf = p.get((B, emb.shape[1]), ctx.dtype)
+            ops.f32_to_16(emb, emb_bf)
             ops.gemm(emb_bf, self._emb_w, ctx.emb_all, bias=self._emb_b)
             p.put(emb_bf)
         else:
@@ -606,7 +623,7 @@ class _UNetBase(nn.Module):
         p.put(temb, h1, e_t, h2, emb)
         ctx.kv_owned = ctx_kv is None
         if ctx_kv is None:
-            ctx_kv = self.project_context(context_bf16, p.get((B * Lctx, self._ctx_kv_cols)))
+            ctx_kv = self.project_context(context_16, p.get((B * Lctx, self._ctx_kv_cols), ctx.dtype))
         ctx.ctx_kv = ctx_kv
         ctx.Lctx = Lctx
 
@@ -628,10 +645,10 @@ class GLVControl(_UNetBase):
                            num_head_channels, transformer_depth, context_dim, adm_in_channels, num_classes, kw)
         self.input_hint_block = TimestepEmbedSequential(ConvIn(in_channels, model_channels, 3, padding=1))
 
-    def run(self, ctx, control_x, t_f32, xt, context_bf16, Lctx, y_f32, ctx_kv=None):
+    def run(self, ctx, control_x, t_f32, xt, context_16, Lctx, y_f32, ctx_kv=None):
         """control_x, xt: fp32 NCHW. Returns list[Act] (the reference's `hs`)."""
         B = xt.shape[0]
-        self._prepare_ctx(ctx, t_f32, context_bf16, B, Lctx, y_f32, ctx_kv)
+        self._prepare_ctx(ctx, t_f32, context_16, B, Lctx, y_f32, ctx_kv)
         hint = self.input_hint_block[0].run_nchw(ctx, control_x)
         h = self.input_blocks[0][0].run_nchw(ctx, xt, residual=hint)   # conv_in(xt) + guided_hint
         ctx.free(hint)
@@ -681,19 +698,19 @@ class LightGLVUNet(_UNetBase):
         for i in [6, 3]:
             self.project_modules.insert(i, ZeroCrossAttn(cond_output_channels[i], concat_channels[i]))
 
-    def pack(self):
-        super().pack()
+    def pack(self, dtype=BF16):
+        super().pack(dtype)
         pack_norm(self.out[0])
         w = self.out[2].weight.detach()
-        self._wout = w.to(BF16).to(torch.float32).permute(0, 2, 3, 1).contiguous()     # [Cout, 3, 3, Cin]
-        self._bout = _bias_bf16_values(self.out[2].bias)
-        self._out_packed = ops.pack_small_cout_weight(w, self.out[2].bias)
+        self._wout = w.to(dtype).to(torch.float32).permute(0, 2, 3, 1).contiguous()     # [Cout, 3, 3, Cin]
+        self._bout = _bias_values(self.out[2].bias, dtype)
+        self._out_packed = ops.pack_small_cout_weight(w, self.out[2].bias, dtype)
         return self
 
-    def run(self, ctx, x, t_f32, context_bf16, Lctx, y_f32, control, out_nchw, ctx_kv=None):
+    def run(self, ctx, x, t_f32, context_16, Lctx, y_f32, control, out_nchw, ctx_kv=None):
         """x fp32 NCHW; control: list[Act] from GLVControl.run; out_nchw: fp32 [B, out_channels, H, W]."""
         B = x.shape[0]
-        self._prepare_ctx(ctx, t_f32, context_bf16, B, Lctx, y_f32, ctx_kv)
+        self._prepare_ctx(ctx, t_f32, context_16, B, Lctx, y_f32, ctx_kv)
         h = self.input_blocks[0][0].run_nchw(ctx, x)
         hs = [h]
         for blk in list(self.input_blocks)[1:]:

@@ -3,6 +3,9 @@
 PyTorch owns every buffer (weights, activations, RNG); kernels run on torch's current CUDA stream so that calls can be
 captured into CUDA graphs. Channels-last activations are 2-D bf16 tensors [B*H*W, C] whose row stride is the leading
 dimension handed to the kernels (column slices of wider buffers are fine).
+
+The ops the diffusion networks use also take fp16 operands (their fp16 compute mode): each picks the bf16 entry point or its
+`_f16` twin from the dtype of its 16-bit operands, and refuses operands that mix the two before anything is launched.
 """
 import ctypes
 
@@ -11,13 +14,27 @@ import torch
 from . import _native
 import os
 
-from ._native import ConvGeometry, Epilogue, call
+from ._native import ConvGeometry, Epilogue
 
 # strided / sub-pixel convolutions through the implicit-GEMM kernel's geometry mode (supir_conv_geom_bf16); "0" restores the
 # im2col buffer (stride 2) and the materialised nearest-2x upsample in front of a plain 3x3 convolution
 CONV_GEOM = os.environ.get("SUPIR_B200_CONV_GEOM", "1") != "0"
 
 BF16 = torch.bfloat16
+F16 = torch.float16
+
+
+def call(name, *args):
+    return _native.call(name, *args)
+
+
+def _entry(name, *ts):
+    """`name` (a bf16 entry point) or its fp16 twin, from the dtype of the 16-bit tensors among `ts` (None and fp32 are
+    ignored). Mixing bf16 and fp16 operands in one call is an error."""
+    dts = {t.dtype for t in ts if t is not None and t.dtype in (BF16, F16)}
+    if len(dts) > 1:
+        raise TypeError(f"{name}: operands mix bfloat16 and float16")
+    return _native.F16_TWINS[name] if dts == {F16} else name
 
 
 def _ptr(t):
@@ -36,6 +53,12 @@ def _need_cuda(*ts):
 
 def _mat(t, dtype=BF16):
     assert t.dim() == 2 and t.stride(1) == 1 and t.dtype == dtype, (t.shape, t.stride(), t.dtype)
+    return t
+
+
+def _mat16(t):
+    """A row-major matrix of 16-bit values (bf16 or fp16)."""
+    assert t.dim() == 2 and t.stride(1) == 1 and t.dtype in (BF16, F16), (t.shape, t.stride(), t.dtype)
     return t
 
 
@@ -98,43 +121,47 @@ def _epilogue(bias, rowvec, rows_per_batch, residual, act, out_f32, ln=None):
 def gemm(a, w, out, bias=None, rowvec=None, rows_per_batch=0, residual=None, act=0, ln=None):
     """out[M, N'] = epilogue(a[M, K] @ w[N, K]^T); N' = N/2 for act=2 (GEGLU). `out` may be fp32 or bf16.
     `ln=(stats, colsum)` folds a LayerNorm of `a` into the epilogue (see supir_epilogue in include/supir_b200.h): `a` is the
-    raw activation, `w` carries gamma, `bias` carries W beta + bias, stats comes from layernorm_stats()."""
+    raw activation, `w` carries gamma, `bias` carries W beta + bias, stats comes from layernorm_stats().
+    a / w / residual / a 16-bit out are all bf16 or all fp16."""
+    name = _entry("supir_gemm_bf16", a, w, out, residual)
     _need_cuda(a, w, out)
-    _mat(a), _mat(w)
+    _mat16(a), _mat16(w)
     M, K = a.shape
     N = w.shape[0]
     assert w.shape[1] == K and out.shape[0] == M and out.shape[1] == (N // 2 if act == 2 else N), (a.shape, w.shape, out.shape)
     if ln is not None:
         assert ln[0].dtype == torch.float32 and ln[0].shape == (M, 2) and ln[0].is_contiguous() and ln[1].shape == (N,)
     ep = _epilogue(bias, rowvec, rows_per_batch, residual, act, out.dtype == torch.float32, ln)
-    call("supir_gemm_bf16", _ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(out), out.stride(0), M, N, K,
+    call(name, _ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(out), out.stride(0), M, N, K,
          ctypes.byref(ep), _stream())
     return out
 
 
 def conv3x3(x, B, H, W, wp, out, bias=None, rowvec=None, residual=None, act=0):
     """3x3/s1/p1 conv on NHWC: x [B*H*W, Cin] (row stride = ld), wp [Cout, 9*Cin] packed (kh, kw, cin)."""
+    name = _entry("supir_conv3x3_bf16", x, wp, out, residual)
     _need_cuda(x, wp, out)
-    _mat(x), _mat(wp)
+    _mat16(x), _mat16(wp)
     Cin = x.shape[1]
     Cout = wp.shape[0]
     assert x.shape[0] == B * H * W and wp.shape[1] == 9 * Cin and wp.is_contiguous() and out.shape == (B * H * W, Cout)
     ep = _epilogue(bias, rowvec, 0, residual, act, out.dtype == torch.float32)
-    call("supir_conv3x3_bf16", _ptr(x), x.stride(0), _ptr(wp), _ptr(out), out.stride(0), B, H, W, Cin, Cout,
+    call(name, _ptr(x), x.stride(0), _ptr(wp), _ptr(out), out.stride(0), B, H, W, Cin, Cout,
          ctypes.byref(ep), _stream())
     return out
 
 
 def conv_geom(x, B, Hin, Win, wp, out, geom, bias=None, act=0):
     """General small-kernel convolution (see supir_conv_geometry): x [B*Hin*Win, Cin], wp [Cout, kh*kw*Cin], out [B*out_H*out_W, Cout]."""
+    name = _entry("supir_conv_geom_bf16", x, wp, out)
     _need_cuda(x, wp, out)
-    _mat(x), _mat(wp)
+    _mat16(x), _mat16(wp)
     Cin, Cout = x.shape[1], wp.shape[0]
     g = ConvGeometry(**geom)
     assert x.shape[0] == B * Hin * Win and wp.shape[1] == g.kh * g.kw * Cin and wp.is_contiguous()
     assert out.shape == (B * g.out_H * g.out_W, Cout), (out.shape, B, g.out_H, g.out_W, Cout)
     ep = _epilogue(bias, None, 0, None, act, out.dtype == torch.float32)
-    call("supir_conv_geom_bf16", _ptr(x), x.stride(0), _ptr(wp), _ptr(out), out.stride(0), B, Hin, Win, Cin, Cout, ctypes.byref(g),
+    call(name, _ptr(x), x.stride(0), _ptr(wp), _ptr(out), out.stride(0), B, Hin, Win, Cin, Cout, ctypes.byref(g),
          ctypes.byref(ep), _stream())
     return out
 
@@ -148,11 +175,11 @@ def conv3x3_stride2(x, B, H, W, wp, out, pad_lo, bias=None):
     return conv_geom(x, B, H, W, wp, out, geom, bias=bias)
 
 
-def fold_upsample_weights(w):
-    """[Cout, Cin, 3, 3] -> four packed [Cout, 2*2*Cin] bf16 matrices, index py*2+px: a 3x3 convolution of the nearest-2x
+def fold_upsample_weights(w, dtype=BF16):
+    """[Cout, Cin, 3, 3] -> four packed [Cout, 2*2*Cin] `dtype` matrices, index py*2+px: a 3x3 convolution of the nearest-2x
     upsampled image equals, for the output pixels of parity (py, px), a 2x2 convolution of the LOW-resolution image whose taps
     are sums of the 3x3 taps that fall on the same source pixel (rows: py=0 -> {0},{1,2}; py=1 -> {0,1},{2}; same for columns)."""
-    wf = w.detach().to(BF16).to(torch.float32)             # the values the reference's bf16 convolution multiplies
+    wf = w.detach().to(dtype).to(torch.float32)            # the values the reference's 16-bit convolution multiplies
     sets = {0: ((0,), (1, 2)), 1: ((0, 1), (2,))}
     out = []
     for py in (0, 1):
@@ -165,7 +192,7 @@ def fold_upsample_weights(w):
                         for kx in sets[px][b]:
                             acc = acc + wf[:, :, ky, kx]
                     taps.append(acc)                        # [Cout, Cin]
-            out.append(torch.stack(taps, 1).reshape(w.shape[0], -1).to(BF16).contiguous())
+            out.append(torch.stack(taps, 1).reshape(w.shape[0], -1).to(dtype).contiguous())
     return out
 
 
@@ -181,11 +208,12 @@ def upsample2x_conv3x3(x, B, H, W, wfold, out, bias=None):
 
 
 def attention(q, k, v, out, B, heads, Lq, Lk, scale=None):
+    name = _entry("supir_attention_bf16", q, k, v, out)
     _need_cuda(q, k, v, out)
     for t in (q, k, v, out):
-        _mat(t)
+        _mat16(t)
     d = q.shape[1] // heads
-    call("supir_attention_bf16", _ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(out),
+    call(name, _ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(out),
          out.stride(0), B, heads, Lq, Lk, d, float(scale if scale is not None else d ** -0.5), _stream())
     return out
 
@@ -216,10 +244,11 @@ def groupnorm_ws_size(B, HW, C, groups=32):
 
 def groupnorm_stats(x, B, HW, ws, groups=32):
     """ws: float64 workspace of groupnorm_ws_size() elements; ws[:B*groups*2] receives (sum, sumsq) per (image, group)."""
+    name = _entry("supir_groupnorm_stats", x)
     _need_cuda(x, ws)
-    _mat(x)
+    _mat16(x)
     assert ws.dtype == torch.float64
-    call("supir_groupnorm_stats", _ptr(x), x.stride(0), B, HW, x.shape[1], groups, _ptr(ws), ws.numel(), _stream())
+    call(name, _ptr(x), x.stride(0), B, HW, x.shape[1], groups, _ptr(ws), ws.numel(), _stream())
     return ws
 
 
@@ -233,46 +262,50 @@ def groupnorm_merge_tiles(tile_mean, tile_var, weights, mean, var):
 
 
 def groupnorm_apply(x, B, HW, out, gamma, beta, eps, silu, sums=None, mean=None, var=None, groups=32):
+    name = _entry("supir_groupnorm_apply", x, out)
     _need_cuda(x, out)
-    _mat(x), _mat(out)
-    call("supir_groupnorm_apply", _ptr(x), x.stride(0), _ptr(out), out.stride(0), B, HW, x.shape[1], groups, _ptr(sums),
+    _mat16(x), _mat16(out)
+    call(name, _ptr(x), x.stride(0), _ptr(out), out.stride(0), B, HW, x.shape[1], groups, _ptr(sums),
          _ptr(mean), _ptr(var), _ptr(gamma), _ptr(beta), float(eps), int(silu), _stream())
     return out
 
 
 def zerosft_apply(h, skip_raw, C1, gamma_beta, out, B, HW, sums, gn_w, gn_b, eps, control_scale, groups=32):
+    name = _entry("supir_zerosft_apply", h, skip_raw, gamma_beta, out)
     _need_cuda(h, gamma_beta, out, control_scale)
-    call("supir_zerosft_apply", _ptr(h), h.stride(0), _ptr(skip_raw), 0 if skip_raw is None else skip_raw.stride(0), C1,
+    call(name, _ptr(h), h.stride(0), _ptr(skip_raw), 0 if skip_raw is None else skip_raw.stride(0), C1,
          _ptr(gamma_beta), gamma_beta.stride(0), _ptr(out), out.stride(0), B, HW, h.shape[1], groups, _ptr(sums),
          _ptr(gn_w), _ptr(gn_b), float(eps), _ptr(control_scale), _stream())
     return out
 
 
 def layernorm(x, out, gamma, beta, eps=1e-5):
+    name = _entry("supir_layernorm_bf16", x, out)
     _need_cuda(x, out)
-    _mat(x), _mat(out)
-    call("supir_layernorm_bf16", _ptr(x), x.stride(0), _ptr(out), out.stride(0), x.shape[0], x.shape[1], _ptr(gamma),
+    _mat16(x), _mat16(out)
+    call(name, _ptr(x), x.stride(0), _ptr(out), out.stride(0), x.shape[0], x.shape[1], _ptr(gamma),
          _ptr(beta), float(eps), _stream())
     return out
 
 
 def layernorm_stats(x, stats, eps=1e-5):
     """stats[r] = (rstd, mean * rstd) of row r of x (fp32 [rows, 2]) for gemm(..., ln=(stats, colsum))."""
+    name = _entry("supir_layernorm_stats", x)
     _need_cuda(x, stats)
-    _mat(x)
+    _mat16(x)
     assert stats.dtype == torch.float32 and stats.shape == (x.shape[0], 2) and stats.is_contiguous()
-    call("supir_layernorm_stats", _ptr(x), x.stride(0), x.shape[0], x.shape[1], float(eps), _ptr(stats), _stream())
+    call(name, _ptr(x), x.stride(0), x.shape[0], x.shape[1], float(eps), _ptr(stats), _stream())
     return stats
 
 
-def fold_layernorm(w, bias, gamma, beta):
-    """Weights of `Linear(LayerNorm(x))` for the folded form: (bf16 W * gamma, fp32 colsum of that, fp32 W beta + bias)."""
-    wf = w.detach().to(BF16).to(torch.float32)                 # the values the reference's bf16 matmul sees
-    wg = (wf * gamma.detach().to(torch.float32)[None, :]).to(BF16).contiguous()
+def fold_layernorm(w, bias, gamma, beta, dtype=BF16):
+    """Weights of `Linear(LayerNorm(x))` for the folded form: (`dtype` W * gamma, fp32 colsum of that, fp32 W beta + bias)."""
+    wf = w.detach().to(dtype).to(torch.float32)                # the values the reference's 16-bit matmul sees
+    wg = (wf * gamma.detach().to(torch.float32)[None, :]).to(dtype).contiguous()
     colsum = wg.to(torch.float32).sum(dim=1).contiguous()
     b2 = wf @ beta.detach().to(torch.float32)
     if bias is not None:
-        b2 = b2 + bias.detach().to(BF16).to(torch.float32)
+        b2 = b2 + bias.detach().to(dtype).to(torch.float32)
     return wg, colsum, b2.contiguous()
 
 
@@ -285,61 +318,65 @@ def softmax_rows(S, P, cols, scale):
 # ------------------------------------------------------------------------------------------------------------------
 # small convs, data movement, embeddings
 # ------------------------------------------------------------------------------------------------------------------
-def pack_small_cin_weight(w):
-    """[Cout, Cin, 3, 3] -> bf16 [Cout, KP] (k = ci*9 + tap, zero padded to a multiple of 64): GEMM operand of the im2col path."""
+def pack_small_cin_weight(w, dtype=BF16):
+    """[Cout, Cin, 3, 3] -> `dtype` [Cout, KP] (k = ci*9 + tap, zero padded to a multiple of 64): GEMM operand of the im2col path."""
     cout, taps = w.shape[0], w.shape[1] * 9
     kp = (taps + 63) // 64 * 64
-    wp = torch.zeros(cout, kp, dtype=BF16, device=w.device)
-    wp[:, :taps] = w.detach().reshape(cout, taps).to(BF16)
+    wp = torch.zeros(cout, kp, dtype=dtype, device=w.device)
+    wp[:, :taps] = w.detach().reshape(cout, taps).to(dtype)
     return wp
 
 
 def conv3x3_small_cin(x_nchw, w, bias, out, residual=None, w_packed=None, pool=None):
     """x_nchw: fp32 [B, Cin, H, W] view with unit stride along W; out NHWC bf16 [B*H*W, Cout].
-    With `w_packed` (pack_small_cin_weight) and a scratch `pool`, large images go through im2col + the tensor-core GEMM."""
+    With `w_packed` (pack_small_cin_weight) and a scratch `pool`, large images go through im2col + the tensor-core GEMM.
+    `out` (and `residual`, `w_packed`) fp16 selects the fp16 kernels: the input is rounded to fp16 instead of bf16."""
+    name = _entry("supir_conv3x3_small_cin", out, residual, w_packed)
     _need_cuda(x_nchw, w, out)
     B, Cin, H, W = x_nchw.shape
     assert x_nchw.dtype == torch.float32 and x_nchw.stride(3) == 1 and w.dtype == torch.float32 and w.is_contiguous()
     if w_packed is not None and pool is not None and B * H * W >= 16384 and out.shape[1] >= 64:
         kp = w_packed.shape[1]
-        cols = pool.get((B * H * W, kp))
-        call("supir_im2col_3x3_small_cin", _ptr(x_nchw), x_nchw.stride(0), x_nchw.stride(1), x_nchw.stride(2), _ptr(cols),
+        cols = pool.get((B * H * W, kp), w_packed.dtype)
+        call(_entry("supir_im2col_3x3_small_cin", cols), _ptr(x_nchw), x_nchw.stride(0), x_nchw.stride(1), x_nchw.stride(2), _ptr(cols),
              cols.stride(0), B, H, W, Cin, kp, _stream())
         gemm(cols, w_packed, out, bias=bias, residual=residual)
         pool.put(cols)
         return out
-    call("supir_conv3x3_small_cin", _ptr(x_nchw), x_nchw.stride(0), x_nchw.stride(1), x_nchw.stride(2), _ptr(w), _ptr(bias),
+    call(name, _ptr(x_nchw), x_nchw.stride(0), x_nchw.stride(1), x_nchw.stride(2), _ptr(w), _ptr(bias),
          _ptr(residual), 0 if residual is None else residual.stride(0), _ptr(out), out.stride(0), B, H, W, Cin, out.shape[1],
          _stream())
     return out
 
 
-def pack_small_cout_weight(w, bias):
-    """[Cout <= 8, Cin, 3, 3] -> (bf16 [8, 9*Cin] in conv3x3's (kh, kw, cin) order, fp32 bias[8]), zero rows beyond Cout."""
+def pack_small_cout_weight(w, bias, dtype=BF16):
+    """[Cout <= 8, Cin, 3, 3] -> (`dtype` [8, 9*Cin] in conv3x3's (kh, kw, cin) order, fp32 bias[8]), zero rows beyond Cout."""
     cout, cin = w.shape[0], w.shape[1]
-    wp = torch.zeros(8, 9 * cin, dtype=BF16, device=w.device)
-    wp[:cout] = w.detach().permute(0, 2, 3, 1).reshape(cout, -1).to(BF16)
+    wp = torch.zeros(8, 9 * cin, dtype=dtype, device=w.device)
+    wp[:cout] = w.detach().permute(0, 2, 3, 1).reshape(cout, -1).to(dtype)
     b8 = torch.zeros(8, dtype=torch.float32, device=w.device)
     if bias is not None:
-        b8[:cout] = bias.detach().to(BF16).to(torch.float32)
+        b8[:cout] = bias.detach().to(dtype).to(torch.float32)
     return wp, b8
 
 
 def conv3x3_small_cout(x, B, H, W, w, bias, out_nchw, crop=None, packed=None, pool=None):
     """x NHWC bf16 [B*H*W, Cin]; out_nchw fp32 [B, Cout, h, w] view (unit stride along w) receiving the crop window.
-    With `packed` (pack_small_cout_weight) and a scratch `pool`, large images run on the tensor cores (Cout padded to 8)."""
+    With `packed` (pack_small_cout_weight) and a scratch `pool`, large images run on the tensor cores (Cout padded to 8).
+    x (and packed[0]) fp16 selects the fp16 kernels."""
+    name = _entry("supir_conv3x3_small_cout", x, None if packed is None else packed[0])
     _need_cuda(x, w, out_nchw)
-    _mat(x)
+    _mat16(x)
     y0, x0, ch, cw = crop if crop is not None else (0, 0, H, W)
     assert out_nchw.dtype == torch.float32 and out_nchw.stride(3) == 1 and tuple(out_nchw.shape[2:]) == (ch, cw)
     if packed is not None and pool is not None and B * H * W >= 16384 and x.shape[1] % 64 == 0:
-        tmp = pool.get((B * H * W, 8))
+        tmp = pool.get((B * H * W, 8), x.dtype)
         conv3x3(x, B, H, W, packed[0], tmp, bias=packed[1])
-        call("supir_nhwc_bf16_crop_to_nchw_f32", _ptr(tmp), tmp.stride(0), _ptr(out_nchw), out_nchw.stride(0), out_nchw.stride(1),
+        call(_entry("supir_nhwc_bf16_crop_to_nchw_f32", tmp), _ptr(tmp), tmp.stride(0), _ptr(out_nchw), out_nchw.stride(0), out_nchw.stride(1),
              out_nchw.stride(2), B, H, W, out_nchw.shape[1], y0, x0, ch, cw, _stream())
         pool.put(tmp)
         return out_nchw
-    call("supir_conv3x3_small_cout", _ptr(x), x.stride(0), _ptr(w), _ptr(bias), _ptr(out_nchw), out_nchw.stride(0),
+    call(name, _ptr(x), x.stride(0), _ptr(w), _ptr(bias), _ptr(out_nchw), out_nchw.stride(0),
          out_nchw.stride(1), out_nchw.stride(2), B, H, W, x.shape[1], out_nchw.shape[1], y0, x0, ch, cw, _stream())
     return out_nchw
 
@@ -370,7 +407,7 @@ def copy2d(src, dst):
 
 
 def axpy(a, y, out, scale):
-    call("supir_axpy_bf16", _ptr(a), a.stride(0), _ptr(y), y.stride(0), _ptr(out), out.stride(0), a.shape[0], a.shape[1],
+    call(_entry("supir_axpy_bf16", a, y, out), _ptr(a), a.stride(0), _ptr(y), y.stride(0), _ptr(out), out.stride(0), a.shape[0], a.shape[1],
          _ptr(scale), _stream())
     return out
 
@@ -389,9 +426,20 @@ def nhwc_bf16_to_nchw_f32(x, B, C, HW, out):
 
 
 def f32_to_bf16(x, out):
-    assert x.is_contiguous() and out.is_contiguous()
+    assert x.is_contiguous() and out.is_contiguous() and out.dtype == BF16
     call("supir_f32_to_bf16", _ptr(x), _ptr(out), x.numel(), _stream())
     return out
+
+
+def f32_to_f16(x, out):
+    assert x.is_contiguous() and out.is_contiguous() and out.dtype == F16
+    call("supir_f32_to_f16", _ptr(x), _ptr(out), x.numel(), _stream())
+    return out
+
+
+def f32_to_16(x, out):
+    """out = x rounded to out's dtype: f32_to_bf16 or f32_to_f16."""
+    return (f32_to_f16 if out.dtype == F16 else f32_to_bf16)(x, out)
 
 
 def timestep_embedding(t, out):
@@ -400,12 +448,14 @@ def timestep_embedding(t, out):
 
 
 def linear_small_m(x, w, bias, out, silu_in=False, silu_out=False, add=None):
+    """w bf16 or fp16; the input and the result are rounded to w's dtype where autocast would round them."""
+    name = _entry("supir_linear_small_m", w)
     _need_cuda(x, w, out)
-    assert x.dtype == torch.float32 and out.dtype == torch.float32 and w.dtype == BF16 and w.is_contiguous()
+    assert x.dtype == torch.float32 and out.dtype == torch.float32 and w.dtype in (BF16, F16) and w.is_contiguous()
     for r0 in range(0, x.shape[0], 16):     # the kernel keeps <= 16 rows in registers; larger batches go in slices
         xs, os_ = x[r0:r0 + 16], out[r0:r0 + 16]
         ad = None if add is None else add[r0:r0 + 16]
-        call("supir_linear_small_m", _ptr(xs), x.stride(0), _ptr(w), _ptr(bias), _ptr(os_), out.stride(0), xs.shape[0], w.shape[0],
+        call(name, _ptr(xs), x.stride(0), _ptr(w), _ptr(bias), _ptr(os_), out.stride(0), xs.shape[0], w.shape[0],
              w.shape[1], int(silu_in), int(silu_out), _ptr(ad), 0 if ad is None else add.stride(0), _stream())
     return out
 

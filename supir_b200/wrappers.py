@@ -4,6 +4,9 @@ Same surface — `ControlWrapper(diffusion_model, compile_model=False, dtype=...
 `.dtype`, `forward(x, t, c, control_scale=1) -> fp32 [B, 4, h, w]`, state_dict keys `diffusion_model.*` / `control_model.*` —
 but one call is one CUDA-graph replay: GLVControl + LightGLVUNet are captured once per (batch, h, w, context length) with
 static input/output buffers, so the ~2000 kernel launches of a denoiser call cost no Python or launch-API time.
+
+`.dtype` selects the compute dtype of both networks: torch.float16 runs them in fp16 (torch.autocast(float16) numerics, the
+reference's default `diffusion_dtype`), torch.bfloat16 in bf16; any other value (fp32) warns and computes bf16.
 """
 import os
 import warnings
@@ -22,19 +25,20 @@ class _Plan:
 
     def __init__(self, wrapper, B, H, W, Lctx, ctx_dim, y_dim, device):
         self.key = (B, H, W, Lctx)
+        self.dtype = wrapper.compute_dtype
         f32 = dict(dtype=torch.float32, device=device)
         self.x = torch.zeros(B, 4, H, W, **f32)
         self.control = torch.zeros(B, 4, H, W, **f32)
         self.t = torch.zeros(B, **f32)
         self.context = torch.zeros(B * Lctx, ctx_dim, **f32)
-        self.context_bf16 = torch.zeros(B * Lctx, ctx_dim, dtype=torch.bfloat16, device=device)
+        self.context_16 = torch.zeros(B * Lctx, ctx_dim, dtype=self.dtype, device=device)      # in the compute dtype
         self.y = torch.zeros(B, y_dim, **f32)
         self.cs = torch.ones(1, **f32)
         self.out = torch.zeros(B, wrapper.diffusion_model.out_channels, H, W, **f32)
         # text K|V projections of both networks: computed OUTSIDE the captured graph, only when the context changes
         # (it is constant over the sampler steps; attention.py:248-251 recomputes it in every call)
-        self.kv_ctrl = torch.zeros(B * Lctx, wrapper.control_model._ctx_kv_cols, dtype=torch.bfloat16, device=device)
-        self.kv_unet = torch.zeros(B * Lctx, wrapper.diffusion_model._ctx_kv_cols, dtype=torch.bfloat16, device=device)
+        self.kv_ctrl = torch.zeros(B * Lctx, wrapper.control_model._ctx_kv_cols, dtype=self.dtype, device=device)
+        self.kv_unet = torch.zeros(B * Lctx, wrapper.diffusion_model._ctx_kv_cols, dtype=self.dtype, device=device)
         self.context_token = None
         self.pool = ops.Pool()
         self.graph = None
@@ -43,16 +47,16 @@ class _Plan:
 
     def project_context(self):
         w = self.wrapper
-        ops.f32_to_bf16(self.context, self.context_bf16)
-        w.control_model.project_context(self.context_bf16, self.kv_ctrl)
-        w.diffusion_model.project_context(self.context_bf16, self.kv_unet)
+        ops.f32_to_16(self.context, self.context_16)
+        w.control_model.project_context(self.context_16, self.kv_ctrl)
+        w.diffusion_model.project_context(self.context_16, self.kv_unet)
 
     def _run(self):
         w = self.wrapper
-        ctx = Ctx(self.pool, self.B)
+        ctx = Ctx(self.pool, self.B, self.dtype)
         ctx.control_scale = self.cs
-        control = w.control_model.run(ctx, self.control, self.t, self.x, self.context_bf16, self.Lctx, self.y, ctx_kv=self.kv_ctrl)
-        w.diffusion_model.run(ctx, self.x, self.t, self.context_bf16, self.Lctx, self.y, control, self.out, ctx_kv=self.kv_unet)
+        control = w.control_model.run(ctx, self.control, self.t, self.x, self.context_16, self.Lctx, self.y, ctx_kv=self.kv_ctrl)
+        w.diffusion_model.run(ctx, self.x, self.t, self.context_16, self.Lctx, self.y, control, self.out, ctx_kv=self.kv_unet)
 
     def build(self):
         self._run()                      # eager warm-up: one-time attribute setup, fills the scratch pool
@@ -81,13 +85,33 @@ class ControlWrapper(nn.Module):
         super().__init__()
         self.diffusion_model = diffusion_model
         self.control_model = None
-        self.dtype = dtype
         self._plans = {}                # (B, H, W, Lctx) -> _Plan, most recently used last
         self.max_plans = int(os.environ.get("SUPIR_B200_MAX_PLANS", "4"))   # each plan owns a captured graph + its activation pool
         self._packed = False
         self._warned = False
         self.replayed_launches = 0      # kernels launched through CUDA-graph replays (supir_launch_count() sees eager ones)
+        self.dtype = dtype
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate())
+
+    @staticmethod
+    def _compute_dtype(dtype):
+        return torch.float16 if dtype == torch.float16 else torch.bfloat16
+
+    @property
+    def dtype(self):
+        """The requested dtype (`diffusion_dtype`): float16 computes in fp16, anything else in bf16."""
+        return self._dtype
+
+    @dtype.setter
+    def dtype(self, value):
+        old = getattr(self, "_dtype", None)
+        self._dtype = value
+        if old is not None and self._compute_dtype(old) != self._compute_dtype(value):
+            self.invalidate()           # packed weights and captured graphs are in the old compute dtype: drop them
+
+    @property
+    def compute_dtype(self):
+        return self._compute_dtype(self._dtype)
 
     def load_control_model(self, control_model):
         self.control_model = control_model
@@ -108,8 +132,8 @@ class ControlWrapper(nn.Module):
         return r
 
     def pack(self):
-        self.diffusion_model.pack()
-        self.control_model.pack()
+        self.diffusion_model.pack(self.compute_dtype)
+        self.control_model.pack(self.compute_dtype)
         self._packed = True
         return self
 
@@ -123,8 +147,8 @@ class ControlWrapper(nn.Module):
             raise RuntimeError("ControlWrapper.forward called before load_control_model()")
         if not x.is_cuda:
             raise RuntimeError("supir_b200.ControlWrapper needs CUDA tensors: the backend has no CPU path")
-        if self.dtype not in (torch.bfloat16,) and not self._warned:
-            warnings.warn(f"supir_b200 computes the diffusion networks in bf16 (requested dtype {self.dtype})")
+        if self.dtype not in (torch.bfloat16, torch.float16) and not self._warned:
+            warnings.warn(f"supir_b200 computes the diffusion networks in bf16 or fp16; dtype {self.dtype} computes in bf16")
             self._warned = True
         if not self._packed:
             self.pack()

@@ -73,12 +73,19 @@ def breakdown(w, B, hw):
 def main():
     if os.environ.get("BENCH_SHAPE_LOG"):
         record_shapes(os.environ["BENCH_SHAPE_LOG"])
-    sizes = [int(a) for a in sys.argv[1:]] or [64, 128]
+    argv = list(sys.argv[1:])
+    dtype = torch.bfloat16
+    if "--dtype" in argv:           # --dtype bf16 | fp16: the compute dtype of the networks
+        i = argv.index("--dtype")
+        dtype = {"bf16": torch.bfloat16, "fp16": torch.float16}[argv[i + 1]]
+        del argv[i:i + 2]
+    sizes = [int(a) for a in argv] or [64, 128]
     t0 = time.time()
     with torch.device("cuda"):
-        unet = nets.LightGLVUNet(mode="XL-base", project_type="ZeroSFT", project_channel_scale=2, **CFG).to(torch.bfloat16)
-        ctrl = nets.GLVControl(input_upscale=1, **CFG).to(torch.bfloat16)
-    w = wrappers.ControlWrapper(unet, dtype=torch.bfloat16)
+        # parameters held in the compute dtype (half the memory of fp32): packing then rounds nothing further
+        unet = nets.LightGLVUNet(mode="XL-base", project_type="ZeroSFT", project_channel_scale=2, **CFG).to(dtype)
+        ctrl = nets.GLVControl(input_upscale=1, **CFG).to(dtype)
+    w = wrappers.ControlWrapper(unet, dtype=dtype)
     w.load_control_model(ctrl)
     w.pack()
     torch.cuda.synchronize()
