@@ -18,9 +18,11 @@
 //   warpgroups 1, 2       : wgmma consumers (m64nBNk16, fp32 accumulators in registers, one wgmma group kept in flight).
 //                   BN in {160, 256}, cooperative: rows [0, 64) and [64, 128) of every tile. BN in {64, 128}, ping-pong: each
 //                   warpgroup owns alternate whole tiles, and one's epilogue runs under the other's mainloop.
-//                   Then the epilogue straight from the accumulator fragment:
-//                   +bias, +per-batch vector (timestep embedding), folded LayerNorm, SiLU / GEGLU, bf16 round, +residual,
-//                   bf16 or fp32 stores. The producer keeps filling the shared-memory ring for the next tile meanwhile.
+//                   Then the epilogue from the accumulator fragment:
+//                   +bias, +per-batch vector (timestep embedding), folded LayerNorm, SiLU / GEGLU, bf16 round, +residual.
+//                   16-bit outputs go through a shared-memory staging buffer and TMA stores (the residual arrives there
+//                   by TMA during the mainloop); fp32 and unaligned outputs are stored directly. The producer keeps
+//                   filling the shared-memory ring for the next tile meanwhile.
 // Pipeline: smem full/empty mbarrier ring (TMA <-> wgmma).
 #include "common.cuh"
 #include "supir_b200.h"
@@ -62,21 +64,44 @@ struct GemmKernelParams {
     int nimg;             // conv mode: number of images
     const float2* ln_stats;  // per-row (rstd, mean * rstd) of A: LayerNorm folded into the epilogue (see supir_epilogue), or null
     const float* ln_colsum;  // [N] row sums of the (gamma-scaled) weight matrix
+    int staged;           // 1: the epilogue goes through shared memory and TMA (tmO / tmR); 0: direct global stores
 };
 
 // tile widths 64 and 128 run the ping-pong schedule (each consumer warpgroup owns whole 128 x BN tiles, BN accumulators per
 // thread); 160 and 256 run the cooperative one (both warpgroups on one tile, BN / 2 accumulators per thread)
 __host__ __device__ constexpr bool gemm_pingpong(int bn) { return bn <= 128; }
 
+// Shared memory: the operand ring, then the staged epilogue's buffer (one per consumer warpgroup: the 128 x BN tile it owns
+// under ping-pong, its 64 x BN half under the cooperative schedule), then the barriers. The ring takes as many stages (<= 8)
+// as fit next to the staging buffers in the 227 KB opt-in limit: 8 / 5 / 5 / 3 stages at BN = 64 / 128 / 160 / 256.
 template <int BN>
 struct GemmSmem {
     static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGES = (192 * 1024) / STAGE_BYTES > 8 ? 8 : (192 * 1024) / STAGE_BYTES;   // 4..8 stages, <= 192 KB
+    static constexpr int FRAG_BYTES = 64 * BN * 2;                                 // one 64-row fragment of 16-bit outputs
+    static constexpr int EPI_BYTES = 2 * (gemm_pingpong(BN) ? 2 : 1) * FRAG_BYTES;  // both consumer warpgroups
     static constexpr int BAR_BYTES = 256;
-    static constexpr int TOTAL = STAGES * STAGE_BYTES + BAR_BYTES + 1024;  // +1024 alignment slack
+    static constexpr int FIT = (227 * 1024 - EPI_BYTES - BAR_BYTES - 1024) / STAGE_BYTES;
+    static constexpr int STAGES = FIT > 8 ? 8 : FIT;
+    static constexpr int TOTAL = STAGES * STAGE_BYTES + EPI_BYTES + BAR_BYTES + 1024;  // +1024 alignment slack
+    static_assert(STAGES >= 3 && TOTAL <= 227 * 1024, "GEMM shared memory does not fit");
 };
+
+// Staged epilogue layout: a 64-row fragment is stored as 32-column slabs of 64 rows x 64 bytes, each slab in the 64-byte
+// swizzle of a SWIZZLE_64B tensor map (16-byte chunk index XOR (row / 2) % 4), so the accumulator fragment's column-pair
+// writes are free of bank conflicts and one TMA box moves one slab. Byte offset of output columns (c, c + 1) of row r:
+__device__ __forceinline__ uint32_t stage_off(int r, int c) {
+    return (c >> 5) * 4096 + r * 64 + ((((c >> 3) & 3) ^ ((r >> 1) & 3)) << 4) + (c & 7) * 2;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v));
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+    return v;
+}
 
 template <int BN, class E>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint64_t db, int scale_d) {
@@ -134,155 +159,150 @@ __device__ __forceinline__ EpiRow epi_row(const GemmKernelParams& p, int mt, int
     return r;
 }
 
-// Epilogue of one m64 accumulator fragment of tile (mt, nt): this thread's rows r_lo and r_lo + 8, columns 8 j + cq (+1).
-// CH > 1: the columns go in chunks of CH pairs (GEGLU: 2 groups of 32 when CH >= 8, else 1), and every global load of a chunk
-// (residual, bias, per-image vector, LN column sums) is issued before its first store, so a chunk waits for one memory latency
-// instead of one per column pair. CH == 1: one pair at a time (the cooperative 256-wide tile, see pick_bn).
-template <int BN, int CH, class E>
-__device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const float (&acc)[BN / 2], int mt, int nt, int r_lo, int cq) {
+// Epilogue of one m64 accumulator fragment of tile (mt, nt): rows [row0, row0 + 64) of the tile, of which this thread holds
+// rows row0 + r_lo and row0 + r_lo + 8, columns 8 j + cq (+1). STAGED: the residual is read from, and the output written to,
+// the fragment's staging buffer at shared address `frag` (stage_off layout; the residual was put there by TMA), and TMA stores
+// it afterwards; rows and columns outside the output are skipped here and clipped by the store. Otherwise both go straight
+// to global memory. The arithmetic and its rounding points are the same either way.
+template <int BN, bool STAGED, class E>
+__device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const float (&acc)[BN / 2], int mt, int nt, int row0,
+                                             int r_lo, int cq, uint32_t frag) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const EpiRow row = epi_row(p, mt, r_lo + 8 * h);
+        const int r = r_lo + 8 * h;
+        const EpiRow row = epi_row(p, mt, row0 + r);
         if (!row.ok) continue;
         const long long grow = row.grow;
         const float* rv = p.rowvec ? p.rowvec + (long long)row.batch * p.rowvec_ld : nullptr;
         if (p.act == 2) {
             // GEGLU: accumulator columns come in groups of 32 = [16 value | 16 gate]; this thread holds value column
             // 8 b + cq (+1) of group g in block 4 g + b and its gate 16 columns later in block 4 g + b + 2
-            constexpr int NG = BN / 32, GCH = CH >= 8 ? 2 : 1;
+            constexpr int NG = BN / 32;
 #pragma unroll
-            for (int g0 = 0; g0 < NG; g0 += GCH) {
-                if (nt * BN + g0 * 32 >= p.N) break;
-                float bx[GCH][2][4], rx[GCH][2][4];
-                uint32_t res[GCH][2];
+            for (int g = 0; g < NG; ++g) {
+                if (nt * BN + g * 32 >= p.N) break;
 #pragma unroll
-                for (int gi = 0; gi < GCH; ++gi) {
-                    const int g = g0 + gi;
-                    const bool gok = g < NG && nt * BN + g * 32 < p.N;
-#pragma unroll
-                    for (int b = 0; b < 2; ++b) {
-                        const int nv = nt * BN + g * 32 + b * 8 + cq;
-                        const int offs[4] = {0, 1, 16, 17};
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            bx[gi][b][e] = (gok && p.bias) ? __ldg(p.bias + nv + offs[e]) : 0.f;
-                            rx[gi][b][e] = (gok && rv) ? __ldg(rv + nv + offs[e]) : 0.f;
-                        }
-                        const int oc = (nt * BN) / 2 + g * 16 + b * 8 + cq;
-                        res[gi][b] = (gok && p.residual) ? load_res_bits<E>(p, grow, oc, true) : 0u;
+                for (int b = 0; b < 2; ++b) {
+                    const int nv = nt * BN + g * 32 + b * 8 + cq;
+                    float xv0 = acc[4 * (4 * g + b) + 2 * h], xv1 = acc[4 * (4 * g + b) + 2 * h + 1];
+                    float gv0 = acc[4 * (4 * g + b + 2) + 2 * h], gv1 = acc[4 * (4 * g + b + 2) + 2 * h + 1];
+                    if (p.bias) {
+                        xv0 += __ldg(p.bias + nv); xv1 += __ldg(p.bias + nv + 1);
+                        gv0 += __ldg(p.bias + nv + 16); gv1 += __ldg(p.bias + nv + 17);
                     }
-                }
-#pragma unroll
-                for (int gi = 0; gi < GCH; ++gi) {
-                    const int g = g0 + gi;
-                    if (g >= NG || nt * BN + g * 32 >= p.N) break;
-#pragma unroll
-                    for (int b = 0; b < 2; ++b) {
-                        float xv0 = acc[4 * (4 * g + b) + 2 * h], xv1 = acc[4 * (4 * g + b) + 2 * h + 1];
-                        float gv0 = acc[4 * (4 * g + b + 2) + 2 * h], gv1 = acc[4 * (4 * g + b + 2) + 2 * h + 1];
-                        if (p.bias) {
-                            xv0 += bx[gi][b][0]; xv1 += bx[gi][b][1];
-                            gv0 += bx[gi][b][2]; gv1 += bx[gi][b][3];
-                        }
-                        if (rv) {
-                            xv0 += rx[gi][b][0]; xv1 += rx[gi][b][1];
-                            gv0 += rx[gi][b][2]; gv1 += rx[gi][b][3];
-                        }
-                        float o0 = E::round(E::round(xv0) * E::round(gelu_erf_f(E::round(gv0))));
-                        float o1 = E::round(E::round(xv1) * E::round(gelu_erf_f(E::round(gv1))));
-                        const int oc = (nt * BN) / 2 + g * 16 + b * 8 + cq;
-                        if (p.residual) {
-                            const float2 r = E::unpack2(res[gi][b]);
-                            o0 += r.x; o1 += r.y;
-                        }
-                        store_pair<E>(p, grow, oc, o0, o1, true);
+                    if (rv) {
+                        xv0 += __ldg(rv + nv); xv1 += __ldg(rv + nv + 1);
+                        gv0 += __ldg(rv + nv + 16); gv1 += __ldg(rv + nv + 17);
                     }
+                    float o0 = E::round(E::round(xv0) * E::round(gelu_erf_f(E::round(gv0))));
+                    float o1 = E::round(E::round(xv1) * E::round(gelu_erf_f(E::round(gv1))));
+                    const int c = g * 16 + b * 8 + cq;                 // output column within the tile's BN / 2
+                    const int oc = (nt * BN) / 2 + c;
+                    if (p.residual) {
+                        const float2 rr = E::unpack2(STAGED ? ld_shared_u32(frag + stage_off(r, c)) : load_res_bits<E>(p, grow, oc, true));
+                        o0 += rr.x; o1 += rr.y;
+                    }
+                    if constexpr (STAGED) st_shared_u32(frag + stage_off(r, c), E::pack2(o0, o1));
+                    else store_pair<E>(p, grow, oc, o0, o1, true);
                 }
             }
         } else {
             float ln_rs = 1.f, ln_nm = 0.f;
             if (p.ln_stats) { const float2 st = __ldg(p.ln_stats + grow); ln_rs = st.x; ln_nm = st.y; }
             constexpr int NJ = BN / 8;
-            // with nothing to load (QKV projections) the chunked form only adds instructions: it measured up to 35 % slower
-            if (CH == 1 || !(p.ln_stats || p.bias || rv || p.residual)) {
 #pragma unroll
-                for (int j = 0; j < NJ; ++j) {
-                    const int n = nt * BN + 8 * j + cq;
-                    if (n >= p.N) break;
-                    const bool n1ok = n + 1 < p.N;
-                    float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-                    if (p.ln_stats) {
-                        v0 = fmaf(v0, ln_rs, -ln_nm * __ldg(p.ln_colsum + n));
-                        if (n1ok) v1 = fmaf(v1, ln_rs, -ln_nm * __ldg(p.ln_colsum + n + 1));
-                    }
-                    if (p.bias) { v0 += __ldg(p.bias + n); if (n1ok) v1 += __ldg(p.bias + n + 1); }
-                    if (rv) { v0 += __ldg(rv + n); if (n1ok) v1 += __ldg(rv + n + 1); }
-                    if (p.act == 1) { v0 = silu_f(E::round(v0)); v1 = silu_f(E::round(v1)); }
-                    if (p.residual) {
-                        const float2 r = E::unpack2(load_res_bits<E>(p, grow, n, n1ok));
-                        if (p.out_f32) { v0 += r.x; v1 += r.y; }
-                        else { v0 = E::round(v0) + r.x; v1 = E::round(v1) + r.y; }
-                    }
-                    store_pair<E>(p, grow, n, v0, v1, n1ok);
+            for (int j = 0; j < NJ; ++j) {
+                const int n = nt * BN + 8 * j + cq;
+                if (n >= p.N) break;
+                const bool n1ok = n + 1 < p.N;
+                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                if (p.ln_stats) {
+                    v0 = fmaf(v0, ln_rs, -ln_nm * __ldg(p.ln_colsum + n));
+                    if (n1ok) v1 = fmaf(v1, ln_rs, -ln_nm * __ldg(p.ln_colsum + n + 1));
                 }
-            } else
-#pragma unroll
-            for (int j0 = 0; j0 < NJ; j0 += CH) {
-                if (nt * BN + 8 * j0 >= p.N) break;
-                float cs[CH][2], bs[CH][2], rx[CH][2];
-                uint32_t res[CH];
-#pragma unroll
-                for (int c = 0; c < CH; ++c) {
-                    const int n = nt * BN + 8 * (j0 + c) + cq;
-                    const bool ok0 = j0 + c < NJ && n < p.N, ok1 = ok0 && n + 1 < p.N;
-                    cs[c][0] = (ok0 && p.ln_stats) ? __ldg(p.ln_colsum + n) : 0.f;
-                    cs[c][1] = (ok1 && p.ln_stats) ? __ldg(p.ln_colsum + n + 1) : 0.f;
-                    bs[c][0] = (ok0 && p.bias) ? __ldg(p.bias + n) : 0.f;
-                    bs[c][1] = (ok1 && p.bias) ? __ldg(p.bias + n + 1) : 0.f;
-                    rx[c][0] = (ok0 && rv) ? __ldg(rv + n) : 0.f;
-                    rx[c][1] = (ok1 && rv) ? __ldg(rv + n + 1) : 0.f;
-                    res[c] = (ok0 && p.residual) ? load_res_bits<E>(p, grow, n, ok1) : 0u;
+                if (p.bias) { v0 += __ldg(p.bias + n); if (n1ok) v1 += __ldg(p.bias + n + 1); }
+                if (rv) { v0 += __ldg(rv + n); if (n1ok) v1 += __ldg(rv + n + 1); }
+                if (p.act == 1) { v0 = silu_f(E::round(v0)); v1 = silu_f(E::round(v1)); }
+                if (p.residual) {
+                    const float2 rr = E::unpack2(STAGED ? ld_shared_u32(frag + stage_off(r, 8 * j + cq)) : load_res_bits<E>(p, grow, n, n1ok));
+                    if (!STAGED && p.out_f32) { v0 += rr.x; v1 += rr.y; }
+                    else { v0 = E::round(v0) + rr.x; v1 = E::round(v1) + rr.y; }
                 }
-#pragma unroll
-                for (int c = 0; c < CH; ++c) {
-                    const int j = j0 + c;
-                    const int n = nt * BN + 8 * j + cq;
-                    if (j >= NJ || n >= p.N) break;
-                    const bool n1ok = n + 1 < p.N;
-                    float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-                    if (p.ln_stats) {
-                        v0 = fmaf(v0, ln_rs, -ln_nm * cs[c][0]);
-                        if (n1ok) v1 = fmaf(v1, ln_rs, -ln_nm * cs[c][1]);
-                    }
-                    if (p.bias) { v0 += bs[c][0]; if (n1ok) v1 += bs[c][1]; }
-                    if (rv) { v0 += rx[c][0]; if (n1ok) v1 += rx[c][1]; }
-                    if (p.act == 1) { v0 = silu_f(E::round(v0)); v1 = silu_f(E::round(v1)); }
-                    if (p.residual) {
-                        const float2 r = E::unpack2(res[c]);
-                        if (p.out_f32) { v0 += r.x; v1 += r.y; }
-                        else { v0 = E::round(v0) + r.x; v1 = E::round(v1) + r.y; }
-                    }
-                    store_pair<E>(p, grow, n, v0, v1, n1ok);
-                }
+                if constexpr (STAGED) st_shared_u32(frag + stage_off(r, 8 * j + cq), E::pack2(v0, v1));
+                else store_pair<E>(p, grow, n, v0, v1, n1ok);
             }
         }
     }
 }
 
+// TMA coordinates of 64-row fragment f (tile rows [64 f, 64 f + 64)) of m-tile mt: GEMM (row, -), conv (x, y, image). False
+// when the fragment has no row inside the output (the tail of the last m-tile, or a conv patch half below the image).
+__device__ __forceinline__ bool frag_origin(const GemmKernelParams& p, int mt, int f, int& c1, int& c2, int& c3) {
+    if (p.conv) {
+        const int per_img = p.tiles_x * p.tiles_y;
+        const int t = mt % per_img;
+        c1 = (t % p.tiles_x) * p.TW + (64 * f) % p.TW;
+        c2 = (t / p.tiles_x) * p.TH + (64 * f) / p.TW;
+        c3 = mt / per_img;
+        return c1 < p.W && c2 < p.H;
+    }
+    c1 = mt * BM + 64 * f;
+    c2 = c3 = 0;
+    return c1 < p.M;
+}
+
+// One thread's TMA traffic for the staging buffer at `buf` (fragments f0 .. f0 + nfrag - 1 of tile (mt, nt), one per
+// FRAG_BYTES): with `bar`, load the residual slabs into it (if the epilogue has a residual: tmR is only valid then) and
+// arrive on `bar` with their byte count (zero bytes completes the phase at once); without, store the output slabs and
+// commit them as one bulk group.
+template <int BN>
+__device__ __forceinline__ void epi_tma(const GemmKernelParams& p, const CUtensorMap* tm, uint8_t* buf, int f0, int nfrag, int mt,
+                                        int nt, uint64_t* bar) {
+    const int bno = p.act == 2 ? BN / 2 : BN;
+    uint32_t bytes = 0;
+    if (bar) {
+        for (int f = 0; f < nfrag && p.residual; ++f) {
+            int c1, c2, c3;
+            if (!frag_origin(p, mt, f0 + f, c1, c2, c3)) continue;
+            for (int s = 0; s < bno / 32 && nt * bno + 32 * s < p.n_out; ++s) bytes += 4096;
+        }
+        mbar_expect_tx(bar, bytes);
+        if (bytes == 0) return;
+    }
+    for (int f = 0; f < nfrag; ++f) {
+        int c1, c2, c3;
+        if (!frag_origin(p, mt, f0 + f, c1, c2, c3)) continue;
+        for (int s = 0; s < bno / 32; ++s) {
+            const int c0 = nt * bno + 32 * s;
+            if (c0 >= p.n_out) break;
+            uint8_t* slab = buf + f * GemmSmem<BN>::FRAG_BYTES + s * 4096;
+            if (bar) {
+                if (p.conv) tma_load_4d(slab, tm, bar, c0, c1, c2, c3);
+                else tma_load_2d(slab, tm, bar, c0, c1);
+            } else {
+                if (p.conv) tma_store_4d(tm, slab, c0, c1, c2, c3);
+                else tma_store_2d(tm, slab, c0, c1);
+            }
+        }
+    }
+    if (!bar) bulk_commit_group();
+}
+
 template <int BN, class E>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKernelParams p) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR, const GemmKernelParams p) {
     using S = GemmSmem<BN>;
     constexpr int STAGES = S::STAGES;
     constexpr bool PINGPONG = gemm_pingpong(BN);
-    // epilogue chunk (see epilogue_m64): 4 pairs when 128 accumulators per thread are live, to stay within 168 registers
-    constexpr int EPI_CH = BN == 256 ? 1 : (PINGPONG && BN == 128 ? 4 : 8);
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + STAGES * S::A_BYTES;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES);   // [STAGES]
+    uint8_t* smem_epi = smem + STAGES * S::STAGE_BYTES;                                  // [2][EPI_BYTES / 2]
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_epi + S::EPI_BYTES);          // [STAGES]
     uint64_t* empty_bar = full_bar + STAGES;                                              // [STAGES]
+    uint64_t* epi_bar = empty_bar + STAGES;                                               // [2]: staging buffer ready
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -291,10 +311,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
+        if (p.staged) {
+            tma_prefetch_desc(&tmO);
+            if (p.residual) tma_prefetch_desc(&tmR);
+        }
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], PINGPONG ? 4 : 8);   // one arrive per warp of the warpgroup(s) consuming the stage
         }
+        mbar_init(&epi_bar[0], 1);
+        mbar_init(&epi_bar[1], 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -347,6 +373,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int wg = (warp - 4) >> 2;
         const int r_w = (warp & 3) * 16 + (lane >> 2);        // this thread's accumulator rows r_w and r_w + 8 of an m64 fragment
         const int cq = 2 * (lane & 3);                        // first of the two columns this thread holds per 8-column block
+        // Staged epilogue: warpgroup wg owns staging buffer wg; its first thread (the leader) issues the buffer's TMA traffic.
+        // Early in each tile's mainloop (after the first k-block's wgmma is issued, so the wait overlaps the tensor cores) the
+        // leader waits until the previous tile's stores have read the buffer, then loads this tile's residual into it and
+        // arrives on epi_bar[wg]; the epilogue waits on that barrier, writes its results over the residual, and the leader
+        // stores them. The operand producer never waits on the staging buffer.
+        uint8_t* ebuf = smem_epi + wg * (S::EPI_BYTES / 2);
+        const bool leader = (threadIdx.x & 127) == 0;
+        uint32_t epi_phase = 0;
+        const int prefetch_kb = p.num_kb > 1 ? 1 : 0;
         if constexpr (PINGPONG) {
             // Ping-pong: warpgroup wg owns the CTA's tiles wg, wg + 2, ... (all 128 rows, two m64 fragments). Their mainloops
             // take turns on the tensor cores through named barriers 1 and 2 (warpgroup wg waits on 1 + wg before its
@@ -374,6 +409,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         wgmma_tile<BN, E>(acc[1], wgmma_desc_sw128(a_addr + 64 * 128 + 32 * k), db, (kb | k) != 0);
                     }
                     wgmma_commit();
+                    if (kb == prefetch_kb && p.staged) {
+                        if (leader) {
+                            bulk_wait_group_read<0>();
+                            epi_tma<BN>(p, &tmR, ebuf, 0, 2, mt, nt, &epi_bar[wg]);
+                        }
+                        __syncwarp();                        // wgmma.wait_group below is warp-aligned
+                    }
                     wgmma_wait<1>();
                     if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
                     prev = stage;
@@ -386,8 +428,20 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 if (lane == 0) mbar_arrive(&empty_bar[prev]);
                 if (tile + (int)gridDim.x < num_tiles) named_bar_arrive(1 + (wg ^ 1), 256);   // the other warpgroup's turn
                 it += 2 * p.num_kb;
-                epilogue_m64<BN, EPI_CH, E>(p, acc[0], mt, nt, r_w, cq);
-                epilogue_m64<BN, EPI_CH, E>(p, acc[1], mt, nt, 64 + r_w, cq);
+                if (p.staged) {
+                    mbar_wait(&epi_bar[wg], epi_phase);
+                    epi_phase ^= 1;
+                    epilogue_m64<BN, true, E>(p, acc[0], mt, nt, 0, r_w, cq, smem_u32(ebuf));
+                    epilogue_m64<BN, true, E>(p, acc[1], mt, nt, 64, r_w, cq, smem_u32(ebuf + S::FRAG_BYTES));
+                    fence_proxy_async_smem();
+                    __syncwarp();
+                    named_bar_sync(3 + wg, 128);
+                    if (leader) epi_tma<BN>(p, &tmO, ebuf, 0, 2, mt, nt, nullptr);
+                    __syncwarp();
+                } else {
+                    epilogue_m64<BN, false, E>(p, acc[0], mt, nt, 0, r_w, cq, 0);
+                    epilogue_m64<BN, false, E>(p, acc[1], mt, nt, 64, r_w, cq, 0);
+                }
             }
         } else {
             // Cooperative: both warpgroups work on every tile, warpgroup wg on rows [64 wg, 64 wg + 64).
@@ -407,6 +461,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     for (int k = 0; k < BK / 16; ++k)       // 16 k-elements = 32 bytes inside the 128B swizzle row
                         wgmma_tile<BN, E>(acc, wgmma_desc_sw128(a_addr + 32 * k), wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
                     wgmma_commit();
+                    if (kb == prefetch_kb && p.staged) {
+                        if (leader) {
+                            bulk_wait_group_read<0>();
+                            epi_tma<BN>(p, &tmR, ebuf, wg, 1, mt, nt, &epi_bar[wg]);
+                        }
+                        __syncwarp();                        // wgmma.wait_group below is warp-aligned
+                    }
                     wgmma_wait<1>();                         // the previous k-block's group has retired: its slot is free
                     if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
                     prev = stage;
@@ -416,9 +477,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 wgmma_fence_operands(acc);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty_bar[prev]);
-                epilogue_m64<BN, EPI_CH, E>(p, acc, mt, nt, wg * 64 + r_w, cq);
+                if (p.staged) {
+                    mbar_wait(&epi_bar[wg], epi_phase);
+                    epi_phase ^= 1;
+                    epilogue_m64<BN, true, E>(p, acc, mt, nt, wg * 64, r_w, cq, smem_u32(ebuf));
+                    fence_proxy_async_smem();
+                    __syncwarp();
+                    named_bar_sync(3 + wg, 128);
+                    if (leader) epi_tma<BN>(p, &tmO, ebuf, wg, 1, mt, nt, nullptr);
+                    __syncwarp();
+                } else {
+                    epilogue_m64<BN, false, E>(p, acc, mt, nt, wg * 64, r_w, cq, 0);
+                }
             }
         }
+        if (p.staged && leader) bulk_wait_group_read<0>();   // the last stores have read the buffer before the CTA exits
     }
 }
 
@@ -526,7 +599,8 @@ int device_sm_count() {
 extern int g_force_bn;
 
 template <int BN, class E>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKernelParams p, cudaStream_t st) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmR,
+                       GemmKernelParams p, cudaStream_t st) {
     using S = GemmSmem<BN>;
     static bool attr_set[64] = {};
     const int dslot = current_device_slot();
@@ -535,7 +609,6 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKerne
         attr_set[dslot] = true;
     }
     p.num_n_tiles = (p.N + BN - 1) / BN;
-    p.nimg = p.conv ? (int)(p.M / ((long long)p.H * p.W)) : 0;
     {
         // tile order that minimises HBM traffic under a simple L2 model (50 MB of L2 on H100): the tiles in flight together
         // (one round: one per SM, two under ping-pong) either share a W tile (m-fastest; A is re-streamed once per n-tile
@@ -551,7 +624,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKerne
     const int tiles = p.num_m_tiles * p.num_n_tiles;
     const int slots = device_sm_count();
     const int grid = tiles < slots ? tiles : slots;
-    gemm_wgmma_kernel<BN, E><<<grid, GEMM_THREADS, S::TOTAL, st>>>(tmA, tmB, p);
+    gemm_wgmma_kernel<BN, E><<<grid, GEMM_THREADS, S::TOTAL, st>>>(tmA, tmB, tmO, tmR, p);
     count_launch();
     SUPIR_CHECK_CUDA(cudaGetLastError());
     return SUPIR_OK;
@@ -564,7 +637,9 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKerne
 // N = 1280), where the mainloop dominates; overhead from the K = 640 residual GEMM (M = 135168, N = 640), where the epilogue
 // and pipeline fill dominate. Under ping-pong (64, 128) the overhead is what the other warpgroup's mainloop does not hide.
 // GEGLU takes the 128-wide ping-pong tile: it was the fastest width on both GEGLU shapes of the step (its epilogue does the
-// most arithmetic per column and hides best under the other warpgroup's mainloop).
+// most arithmetic per column and hides best under the other warpgroup's mainloop). Re-checked with the staged epilogue by
+// tools/bench_gemm_widths.py on an H100 80GB HBM3 at 400 W (1695-1800 MHz under sw_power_cap): the widths this model picks
+// total 604.3 ms per 34-row denoiser call against 604.2 ms for the fastest width of every shape, so the constants stand.
 static int pick_bn(const GemmKernelParams& p, int force_bn) {
     const int m_tiles = p.num_m_tiles, N = p.N, num_kb = p.num_kb;
     if (force_bn == 64 || force_bn == 128 || force_bn == 160 || force_bn == 256) return force_bn;
@@ -588,13 +663,55 @@ static int pick_bn(const GemmKernelParams& p, int force_bn) {
 
 int g_force_bn = 0;
 
+// The staged epilogue needs what TMA can address: a 16-bit output and residual with 16-byte aligned base pointers and row
+// strides (fp32 outputs of the text towers, odd leading dimensions and odd-address residuals take the direct stores), and
+// a whole number of 32-column slabs per tile (not GEGLU at width 160, 80 output columns, which pick_bn never chooses).
+static bool can_stage(const GemmKernelParams& p, int bn) {
+    const auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    return !p.out_f32 && (p.act != 2 || bn % 64 == 0) && al16(p.out) && (p.ldc * 2) % 16 == 0 &&
+           (!p.residual || (al16(p.residual) && (p.ldr * 2) % 16 == 0));
+}
+
+// Tensor maps of the staged epilogue's output (tmO) and residual (tmR): boxes of 32 columns x 64 rows, 64-byte swizzle (see
+// stage_off). GEMM: 2-D over [M, n_out]. Conv: 4-D over [nimg, H, W, n_out] with the output placement of the geometry (the
+// interleaved sub-pixel outputs start at their offset pixel and step out_sx / out_sy pixels); the box is the 64 pixels of
+// half a TH x TW patch. TMA clips the boxes at the tensor's edges.
+template <class E>
+static int make_epilogue_maps(GemmKernelParams& p, int bn, CUtensorMap* tmO, CUtensorMap* tmR) {
+    p.staged = can_stage(p, bn) ? 1 : 0;
+    if (!p.staged) return SUPIR_OK;
+    using T = typename E::T;
+    if (p.conv) {
+        const uint32_t bw = p.TW < 64 ? p.TW : 64;
+        const uint32_t box[4] = {32, bw, 64 / bw, 1};
+        const uint64_t dims[4] = {(uint64_t)p.n_out, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.nimg};
+        const uint64_t ost[3] = {(uint64_t)(p.ldc * p.out_sx), (uint64_t)(p.ldc * p.out_sy * p.out_W), (uint64_t)(p.ldc * p.out_H * p.out_W)};
+        const T* obase = reinterpret_cast<const T*>(p.out) + ((long long)p.out_oy * p.out_W + p.out_ox) * p.ldc;
+        int rc = make_tmap_16_sw(tmO, E::kTma, obase, 4, dims, ost, box, 64);
+        if (rc || !p.residual) return rc;
+        const uint64_t rst[3] = {(uint64_t)p.ldr, (uint64_t)(p.ldr * p.W), (uint64_t)(p.ldr * p.W * p.H)};
+        return make_tmap_16_sw(tmR, E::kTma, p.residual, 4, dims, rst, box, 64);
+    }
+    const uint32_t box[2] = {32, 64};
+    const uint64_t dims[2] = {(uint64_t)p.n_out, (uint64_t)p.M};
+    const uint64_t ost[1] = {(uint64_t)p.ldc};
+    int rc = make_tmap_16_sw(tmO, E::kTma, p.out, 2, dims, ost, box, 64);
+    if (rc || !p.residual) return rc;
+    const uint64_t rst[1] = {(uint64_t)p.ldr};
+    return make_tmap_16_sw(tmR, E::kTma, p.residual, 2, dims, rst, box, 64);
+}
+
 template <class E>
 static int run_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKernelParams& p, cudaStream_t st) {
+    if (p.conv) p.nimg = (int)(p.M / ((long long)p.H * p.W));
     const int bn = pick_bn(p, g_force_bn);
-    if (bn == 256) return launch_gemm<256, E>(tmA, tmB, p, st);
-    if (bn == 160) return launch_gemm<160, E>(tmA, tmB, p, st);
-    if (bn == 128) return launch_gemm<128, E>(tmA, tmB, p, st);
-    return launch_gemm<64, E>(tmA, tmB, p, st);
+    CUtensorMap tmO{}, tmR{};
+    const int rc = make_epilogue_maps<E>(p, bn, &tmO, &tmR);
+    if (rc) return rc;
+    if (bn == 256) return launch_gemm<256, E>(tmA, tmB, tmO, tmR, p, st);
+    if (bn == 160) return launch_gemm<160, E>(tmA, tmB, tmO, tmR, p, st);
+    if (bn == 128) return launch_gemm<128, E>(tmA, tmB, tmO, tmR, p, st);
+    return launch_gemm<64, E>(tmA, tmB, tmO, tmR, p, st);
 }
 
 static int fill_epilogue(GemmKernelParams& p, const supir_epilogue* ep, int N) {
