@@ -1,4 +1,4 @@
-// supir_b200 — library-level C ABI: error string, version, launch counter.
+// supir_b200 — library-level C ABI: error string, version, launch counter; the per-device plumbing of common.cuh.
 #include "common.cuh"
 #include "supir_b200.h"
 
@@ -20,6 +20,23 @@ int set_error(int code, const char* fmt, ...) {
 }
 
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+
+// current device, clamped into the per-device caches (function attributes and SM counts are per device)
+int current_device_slot() {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    return dev < 0 ? 0 : (dev > 63 ? 63 : dev);
+}
+
+int device_sm_count() {
+    static int sms[64] = {};
+    const int d = current_device_slot();
+    if (sms[d] == 0) {
+        cudaDeviceGetAttribute(&sms[d], cudaDevAttrMultiProcessorCount, d);
+        if (sms[d] <= 0) sms[d] = 132;
+    }
+    return sms[d];
+}
 
 }  // namespace supir
 

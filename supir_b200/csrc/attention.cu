@@ -30,9 +30,6 @@
 
 namespace supir {
 
-int make_tmap_16(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
-                 const uint64_t* strides_elems, const uint32_t* box);
-
 static constexpr int ATT_BM = 128;   // queries per CTA (64 per consumer warpgroup)
 static constexpr int ATT_THREADS = 384;
 

@@ -17,6 +17,11 @@ void count_launch(int n = 1);  // bumps the counter behind supir_launch_count()
 int device_sm_count();
 int current_device_slot();   // cudaGetDevice() clamped to [0, 63]: index of the per-device caches
 
+// Tensor map of 16-bit elements (defined in gemm.cu): dims / strides innermost first, strides in elements; `swizzle` in bytes;
+// `elem_strides` (null: all 1) are TMA traversal strides. Rejects base addresses and strides TMA cannot take.
+int make_tmap_16(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
+                 const uint64_t* strides_elems, const uint32_t* box, int swizzle = 128, const uint32_t* elem_strides = nullptr);
+
 #define SUPIR_OK 0
 #define SUPIR_ERR_INVALID -1
 #define SUPIR_ERR_CUDA -2

@@ -28,7 +28,6 @@
 #include "supir_b200.h"
 #include "wgmma.cuh"
 
-#include <cstdlib>
 #include <mutex>
 
 namespace supir {
@@ -133,6 +132,21 @@ __device__ __forceinline__ uint32_t load_res_bits(const GemmKernelParams& p, lon
     return n1ok ? lo | (E::bits(src[1]) << 16) : lo;
 }
 
+// m-tile and n-tile of persistent tile index `tile` (tile order: m_fastest)
+__device__ __forceinline__ void tile_coords(const GemmKernelParams& p, int tile, int& mt, int& nt) {
+    mt = p.m_fastest ? tile % p.num_m_tiles : tile / p.num_n_tiles;
+    nt = p.m_fastest ? tile / p.num_m_tiles : tile % p.num_n_tiles;
+}
+
+// conv mode: image b and output pixel (y, x) of row r of m-tile mt (its rows are a TH x TW pixel patch, row-major)
+__device__ __forceinline__ void conv_pixel(const GemmKernelParams& p, int mt, int r, int& b, int& y, int& x) {
+    const int per_img = p.tiles_x * p.tiles_y;
+    b = mt / per_img;
+    const int t = mt % per_img;
+    y = (t / p.tiles_x) * p.TH + r / p.TW;
+    x = (t % p.tiles_x) * p.TW + r % p.TW;
+}
+
 // output row of accumulator row `row_in_tile` of m-tile `mt`: its row index in the output / residual, its image (per-batch
 // vector index) and whether it exists
 struct EpiRow {
@@ -143,11 +157,8 @@ struct EpiRow {
 __device__ __forceinline__ EpiRow epi_row(const GemmKernelParams& p, int mt, int row_in_tile) {
     EpiRow r;
     if (p.conv) {
-        const int per_img = p.tiles_x * p.tiles_y;
-        const int b = mt / per_img;
-        const int t = mt % per_img;
-        const int y = (t / p.tiles_x) * p.TH + row_in_tile / p.TW;
-        const int x = (t % p.tiles_x) * p.TW + row_in_tile % p.TW;
+        int b, y, x;
+        conv_pixel(p, mt, row_in_tile, b, y, x);
         r.ok = (y < p.H) && (x < p.W) && (b < p.nimg);
         r.grow = ((long long)b * p.out_H + (long long)y * p.out_sy + p.out_oy) * p.out_W + (long long)x * p.out_sx + p.out_ox;
         r.batch = b;
@@ -239,11 +250,7 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
 // when the fragment has no row inside the output (the tail of the last m-tile, or a conv patch half below the image).
 __device__ __forceinline__ bool frag_origin(const GemmKernelParams& p, int mt, int f, int& c1, int& c2, int& c3) {
     if (p.conv) {
-        const int per_img = p.tiles_x * p.tiles_y;
-        const int t = mt % per_img;
-        c1 = (t % p.tiles_x) * p.TW + (64 * f) % p.TW;
-        c2 = (t / p.tiles_x) * p.TH + (64 * f) / p.TW;
-        c3 = mt / per_img;
+        conv_pixel(p, mt, 64 * f, c3, c2, c1);
         return c1 < p.W && c2 < p.H;
     }
     c1 = mt * BM + 64 * f;
@@ -332,16 +339,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                const int mt = p.m_fastest ? tile % p.num_m_tiles : tile / p.num_n_tiles;
-                const int nt = p.m_fastest ? tile / p.num_m_tiles : tile % p.num_n_tiles;
+                int mt, nt;
+                tile_coords(p, tile, mt, nt);
                 int b = 0, y0 = 0, x0 = 0;
-                if (p.conv) {
-                    const int per_img = p.tiles_x * p.tiles_y;
-                    b = mt / per_img;
-                    const int r = mt % per_img;
-                    y0 = (r / p.tiles_x) * p.TH;
-                    x0 = (r % p.tiles_x) * p.TW;
-                }
+                if (p.conv) conv_pixel(p, mt, 0, b, y0, x0);
                 const int bn0 = nt * BN;
                 // conv mode walks (tap row, tap column, 64-channel chunk) with counters: no division in the per-k-block path
                 int cc = 0, tx = 0, ty = 0, wcol = 0;
@@ -370,125 +371,90 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     } else {
         asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
         // ===================== wgmma consumers + epilogue (warpgroups 1, 2) =====================
-        const int wg = (warp - 4) >> 2;
-        const int r_w = (warp & 3) * 16 + (lane >> 2);        // this thread's accumulator rows r_w and r_w + 8 of an m64 fragment
-        const int cq = 2 * (lane & 3);                        // first of the two columns this thread holds per 8-column block
+        // Two schedules, fixed by the tile width (gemm_pingpong):
+        //   ping-pong (BN 64, 128): warpgroup wg owns the CTA's tiles wg, wg + 2, ... whole (all 128 rows: FRAGS = 2 m64
+        //     fragments). Their mainloops take turns on the tensor cores through named barriers 1 and 2 (warpgroup wg waits
+        //     on 1 + wg before its mainloop; the other arrives on it after finishing its own), so one warpgroup's epilogue
+        //     runs under the other's mainloop. A warpgroup's ring position skips the other's k-blocks. The handoff also keeps
+        //     each warpgroup within one ring pass of the producer, which makes the parity waits on the full barriers
+        //     unambiguous.
+        //   cooperative (BN 160, 256): both warpgroups work on every tile, warpgroup wg on rows [64 wg, 64 wg + 64) (FRAGS =
+        //     1, fragment wg), and both walk the whole ring in step.
         // Staged epilogue: warpgroup wg owns staging buffer wg; its first thread (the leader) issues the buffer's TMA traffic.
         // Early in each tile's mainloop (after the first k-block's wgmma is issued, so the wait overlaps the tensor cores) the
         // leader waits until the previous tile's stores have read the buffer, then loads this tile's residual into it and
         // arrives on epi_bar[wg]; the epilogue waits on that barrier, writes its results over the residual, and the leader
         // stores them. The operand producer never waits on the staging buffer.
+        constexpr int FRAGS = PINGPONG ? 2 : 1;
+        const int wg = (warp - 4) >> 2;
+        const int frag0 = PINGPONG ? 0 : wg;                  // this warpgroup's first m64 fragment of a tile
+        const int r_w = (warp & 3) * 16 + (lane >> 2);        // this thread's accumulator rows r_w and r_w + 8 of an m64 fragment
+        const int cq = 2 * (lane & 3);                        // first of the two columns this thread holds per 8-column block
         uint8_t* ebuf = smem_epi + wg * (S::EPI_BYTES / 2);
         const bool leader = (threadIdx.x & 127) == 0;
         uint32_t epi_phase = 0;
         const int prefetch_kb = p.num_kb > 1 ? 1 : 0;
-        if constexpr (PINGPONG) {
-            // Ping-pong: warpgroup wg owns the CTA's tiles wg, wg + 2, ... (all 128 rows, two m64 fragments). Their mainloops
-            // take turns on the tensor cores through named barriers 1 and 2 (warpgroup wg waits on 1 + wg before its
-            // mainloop; the other arrives on it after finishing its own), so one warpgroup's epilogue runs under the other's
-            // mainloop. The handoff also keeps each warpgroup within one ring pass of the producer, which makes the parity
-            // waits on the full barriers unambiguous.
-            float acc[2][BN / 2];
-            int it = wg * p.num_kb;                           // ring position of this warpgroup's next k-block
-            for (int tile = blockIdx.x + wg * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x) {
-                const int mt = p.m_fastest ? tile % p.num_m_tiles : tile / p.num_n_tiles;
-                const int nt = p.m_fastest ? tile / p.num_m_tiles : tile % p.num_n_tiles;
+        float acc[FRAGS][BN / 2];
+        int it = wg * p.num_kb;                               // ping-pong: ring position of this warpgroup's next k-block
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int tile = blockIdx.x + (PINGPONG ? wg : 0) * gridDim.x; tile < num_tiles; tile += (PINGPONG ? 2 : 1) * gridDim.x) {
+            int mt, nt;
+            tile_coords(p, tile, mt, nt);
+            if constexpr (PINGPONG) {
                 if (tile != (int)blockIdx.x) named_bar_sync(1 + wg, 256);
-                int stage = it % STAGES;
-                uint32_t phase = (it / STAGES) & 1;
-                int prev = -1;
-                for (int kb = 0; kb < p.num_kb; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    const uint32_t a_addr = smem_u32(smem_a + stage * S::A_BYTES);
-                    const uint32_t b_addr = smem_u32(smem_b + stage * S::B_BYTES);
-                    wgmma_fence();
+                stage = it % STAGES;
+                phase = (it / STAGES) & 1;
+            }
+            int prev = -1;
+            for (int kb = 0; kb < p.num_kb; ++kb) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint32_t a_addr = smem_u32(smem_a + stage * S::A_BYTES + frag0 * 64 * 128);
+                const uint32_t b_addr = smem_u32(smem_b + stage * S::B_BYTES);
+                wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        const uint64_t db = wgmma_desc_sw128(b_addr + 32 * k);
-                        wgmma_tile<BN, E>(acc[0], wgmma_desc_sw128(a_addr + 32 * k), db, (kb | k) != 0);
-                        wgmma_tile<BN, E>(acc[1], wgmma_desc_sw128(a_addr + 64 * 128 + 32 * k), db, (kb | k) != 0);
-                    }
-                    wgmma_commit();
-                    if (kb == prefetch_kb && p.staged) {
-                        if (leader) {
-                            bulk_wait_group_read<0>();
-                            epi_tma<BN>(p, &tmR, ebuf, 0, 2, mt, nt, &epi_bar[wg]);
-                        }
-                        __syncwarp();                        // wgmma.wait_group below is warp-aligned
-                    }
-                    wgmma_wait<1>();
-                    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
-                    prev = stage;
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                for (int k = 0; k < BK / 16; ++k) {           // 16 k-elements = 32 bytes inside the 128B swizzle row
+                    const uint64_t db = wgmma_desc_sw128(b_addr + 32 * k);
+#pragma unroll
+                    for (int f = 0; f < FRAGS; ++f)
+                        wgmma_tile<BN, E>(acc[f], wgmma_desc_sw128(a_addr + f * 64 * 128 + 32 * k), db, (kb | k) != 0);
                 }
-                wgmma_wait<0>();
-                wgmma_fence_operands(acc[0]);
-                wgmma_fence_operands(acc[1]);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                wgmma_commit();
+                if (kb == prefetch_kb && p.staged) {
+                    if (leader) {
+                        bulk_wait_group_read<0>();
+                        epi_tma<BN>(p, &tmR, ebuf, frag0, FRAGS, mt, nt, &epi_bar[wg]);
+                    }
+                    __syncwarp();                            // wgmma.wait_group below is warp-aligned
+                }
+                wgmma_wait<1>();                             // the previous k-block's group has retired: its slot is free
+                if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+#pragma unroll
+            for (int f = 0; f < FRAGS; ++f) wgmma_fence_operands(acc[f]);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            if constexpr (PINGPONG) {
                 if (tile + (int)gridDim.x < num_tiles) named_bar_arrive(1 + (wg ^ 1), 256);   // the other warpgroup's turn
                 it += 2 * p.num_kb;
-                if (p.staged) {
-                    mbar_wait(&epi_bar[wg], epi_phase);
-                    epi_phase ^= 1;
-                    epilogue_m64<BN, true, E>(p, acc[0], mt, nt, 0, r_w, cq, smem_u32(ebuf));
-                    epilogue_m64<BN, true, E>(p, acc[1], mt, nt, 64, r_w, cq, smem_u32(ebuf + S::FRAG_BYTES));
-                    fence_proxy_async_smem();
-                    __syncwarp();
-                    named_bar_sync(3 + wg, 128);
-                    if (leader) epi_tma<BN>(p, &tmO, ebuf, 0, 2, mt, nt, nullptr);
-                    __syncwarp();
-                } else {
-                    epilogue_m64<BN, false, E>(p, acc[0], mt, nt, 0, r_w, cq, 0);
-                    epilogue_m64<BN, false, E>(p, acc[1], mt, nt, 64, r_w, cq, 0);
-                }
             }
-        } else {
-            // Cooperative: both warpgroups work on every tile, warpgroup wg on rows [64 wg, 64 wg + 64).
-            float acc[BN / 2];
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                const int mt = p.m_fastest ? tile % p.num_m_tiles : tile / p.num_n_tiles;
-                const int nt = p.m_fastest ? tile / p.num_m_tiles : tile % p.num_n_tiles;
-                int prev = -1;
-                for (int kb = 0; kb < p.num_kb; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    const uint32_t a_addr = smem_u32(smem_a + stage * S::A_BYTES + wg * 64 * 128);
-                    const uint32_t b_addr = smem_u32(smem_b + stage * S::B_BYTES);
-                    wgmma_fence();
+            if (p.staged) {
+                mbar_wait(&epi_bar[wg], epi_phase);
+                epi_phase ^= 1;
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k)       // 16 k-elements = 32 bytes inside the 128B swizzle row
-                        wgmma_tile<BN, E>(acc, wgmma_desc_sw128(a_addr + 32 * k), wgmma_desc_sw128(b_addr + 32 * k), (kb | k) != 0);
-                    wgmma_commit();
-                    if (kb == prefetch_kb && p.staged) {
-                        if (leader) {
-                            bulk_wait_group_read<0>();
-                            epi_tma<BN>(p, &tmR, ebuf, wg, 1, mt, nt, &epi_bar[wg]);
-                        }
-                        __syncwarp();                        // wgmma.wait_group below is warp-aligned
-                    }
-                    wgmma_wait<1>();                         // the previous k-block's group has retired: its slot is free
-                    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
-                    prev = stage;
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-                wgmma_wait<0>();
-                wgmma_fence_operands(acc);
+                for (int f = 0; f < FRAGS; ++f)
+                    epilogue_m64<BN, true, E>(p, acc[f], mt, nt, 64 * (frag0 + f), r_w, cq, smem_u32(ebuf + f * S::FRAG_BYTES));
+                fence_proxy_async_smem();
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&empty_bar[prev]);
-                if (p.staged) {
-                    mbar_wait(&epi_bar[wg], epi_phase);
-                    epi_phase ^= 1;
-                    epilogue_m64<BN, true, E>(p, acc, mt, nt, wg * 64, r_w, cq, smem_u32(ebuf));
-                    fence_proxy_async_smem();
-                    __syncwarp();
-                    named_bar_sync(3 + wg, 128);
-                    if (leader) epi_tma<BN>(p, &tmO, ebuf, wg, 1, mt, nt, nullptr);
-                    __syncwarp();
-                } else {
-                    epilogue_m64<BN, false, E>(p, acc, mt, nt, wg * 64, r_w, cq, 0);
-                }
+                named_bar_sync(3 + wg, 128);
+                if (leader) epi_tma<BN>(p, &tmO, ebuf, frag0, FRAGS, mt, nt, nullptr);
+                __syncwarp();
+            } else {
+#pragma unroll
+                for (int f = 0; f < FRAGS; ++f) epilogue_m64<BN, false, E>(p, acc[f], mt, nt, 64 * (frag0 + f), r_w, cq, 0);
             }
         }
         if (p.staged && leader) bulk_wait_group_read<0>();   // the last stores have read the buffer before the CTA exits
@@ -516,10 +482,12 @@ static PFN_tmapEncodeTiled get_encode_fn() {
     return fn;
 }
 
-// rank-N tensor map of 16-bit elements (bf16 or fp16: `dt`); dims/strides innermost first; strides in ELEMENTS for
-// dims 1..rank-1
-static int make_tmap_16_sw(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
-                           const uint64_t* strides_elems, const uint32_t* box, int swizzle_bytes) {
+// Tensor map of 16-bit elements (bf16 or fp16: `dt`); dims / strides innermost first, strides in ELEMENTS for dims
+// 1..rank-1. `swizzle` in bytes: 128 for GEMM / attention operands, 64 for the staged epilogue's slabs. `elem_strides`
+// (null: all 1) are traversal strides: the box spans box[i] tensor elements of dimension i and delivers every
+// elem_strides[i]-th of them, densely packed (a stride-2 convolution's input patch).
+int make_tmap_16(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
+                 const uint64_t* strides_elems, const uint32_t* box, int swizzle, const uint32_t* elem_strides) {
     PFN_tmapEncodeTiled fn = get_encode_fn();
     if (!fn) return set_error(SUPIR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
     cuuint64_t gdim[5], gstr[4];
@@ -527,7 +495,7 @@ static int make_tmap_16_sw(CUtensorMap* m, CUtensorMapDataType dt, const void* b
     for (int i = 0; i < rank; ++i) {
         gdim[i] = dims[i];
         bx[i] = box[i];
-        es[i] = 1;
+        es[i] = elem_strides ? elem_strides[i] : 1;
     }
     for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_elems[i] * 2;
     if ((reinterpret_cast<uintptr_t>(base) & 15) != 0)
@@ -535,68 +503,16 @@ static int make_tmap_16_sw(CUtensorMap* m, CUtensorMapDataType dt, const void* b
     for (int i = 0; i + 1 < rank; ++i)
         if (gstr[i] % 16 != 0) return set_error(SUPIR_ERR_INVALID, "TMA stride %d (%llu B) not a multiple of 16", i,
                                                  (unsigned long long)gstr[i]);
-    const CUtensorMapSwizzle sw = swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                                  : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                  : swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE;
+    const CUtensorMapSwizzle sw = swizzle == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                  : swizzle == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                  : swizzle == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE;
     CUresult r = fn(m, dt, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(SUPIR_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
+    if (r != CUDA_SUCCESS)
+        return set_error(SUPIR_ERR_CUDA, "cuTensorMapEncodeTiled%s failed with CUresult %d", elem_strides ? " (strided)" : "",
+                         (int)r);
     return SUPIR_OK;
 }
-
-int make_tmap_bf16_sw(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
-                      const uint32_t* box, int swizzle_bytes) {
-    return make_tmap_16_sw(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_elems, box, swizzle_bytes);
-}
-
-// 128B-swizzled map of a GEMM / attention operand
-int make_tmap_16(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
-                 const uint64_t* strides_elems, const uint32_t* box) {
-    return make_tmap_16_sw(m, dt, base, rank, dims, strides_elems, box, 128);
-}
-
-int make_tmap_bf16(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
-                   const uint32_t* box) {
-    return make_tmap_16(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_elems, box);
-}
-
-// same with traversal strides (elementStrides): the box spans box[i] tensor elements of dimension i and delivers every
-// elem_strides[i]-th of them, densely packed (a stride-2 convolution's input patch)
-static int make_tmap_16_strided(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
-                                const uint64_t* strides_elems, const uint32_t* box, const uint32_t* elem_strides) {
-    PFN_tmapEncodeTiled fn = get_encode_fn();
-    if (!fn) return set_error(SUPIR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-    cuuint64_t gdim[5], gstr[4];
-    cuuint32_t bx[5], es[5];
-    for (int i = 0; i < rank; ++i) { gdim[i] = dims[i]; bx[i] = box[i]; es[i] = elem_strides[i]; }
-    for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_elems[i] * 2;
-    if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return set_error(SUPIR_ERR_INVALID, "TMA base address %p is not 16-byte aligned", base);
-    for (int i = 0; i + 1 < rank; ++i)
-        if (gstr[i] % 16 != 0) return set_error(SUPIR_ERR_INVALID, "TMA stride %d (%llu B) not a multiple of 16", i, (unsigned long long)gstr[i]);
-    CUresult r = fn(m, dt, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return set_error(SUPIR_ERR_CUDA, "cuTensorMapEncodeTiled (strided) failed with CUresult %d", (int)r);
-    return SUPIR_OK;
-}
-
-// current device, clamped into the per-device caches below (function attributes and SM counts are per device)
-int current_device_slot() {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    return dev < 0 ? 0 : (dev > 63 ? 63 : dev);
-}
-
-int device_sm_count() {
-    static int sms[64] = {};
-    const int d = current_device_slot();
-    if (sms[d] == 0) {
-        cudaDeviceGetAttribute(&sms[d], cudaDevAttrMultiProcessorCount, d);
-        if (sms[d] <= 0) sms[d] = 132;
-    }
-    return sms[d];
-}
-
-extern int g_force_bn;
 
 template <int BN, class E>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmR,
@@ -661,7 +577,7 @@ static int pick_bn(const GemmKernelParams& p, int force_bn) {
     return best;
 }
 
-int g_force_bn = 0;
+static int g_force_bn = 0;   // supir_set_gemm_tile_n: 0 = pick_bn's choice
 
 // The staged epilogue needs what TMA can address: a 16-bit output and residual with 16-byte aligned base pointers and row
 // strides (fp32 outputs of the text towers, odd leading dimensions and odd-address residuals take the direct stores), and
@@ -687,26 +603,32 @@ static int make_epilogue_maps(GemmKernelParams& p, int bn, CUtensorMap* tmO, CUt
         const uint64_t dims[4] = {(uint64_t)p.n_out, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.nimg};
         const uint64_t ost[3] = {(uint64_t)(p.ldc * p.out_sx), (uint64_t)(p.ldc * p.out_sy * p.out_W), (uint64_t)(p.ldc * p.out_H * p.out_W)};
         const T* obase = reinterpret_cast<const T*>(p.out) + ((long long)p.out_oy * p.out_W + p.out_ox) * p.ldc;
-        int rc = make_tmap_16_sw(tmO, E::kTma, obase, 4, dims, ost, box, 64);
+        int rc = make_tmap_16(tmO, E::kTma, obase, 4, dims, ost, box, 64);
         if (rc || !p.residual) return rc;
         const uint64_t rst[3] = {(uint64_t)p.ldr, (uint64_t)(p.ldr * p.W), (uint64_t)(p.ldr * p.W * p.H)};
-        return make_tmap_16_sw(tmR, E::kTma, p.residual, 4, dims, rst, box, 64);
+        return make_tmap_16(tmR, E::kTma, p.residual, 4, dims, rst, box, 64);
     }
     const uint32_t box[2] = {32, 64};
     const uint64_t dims[2] = {(uint64_t)p.n_out, (uint64_t)p.M};
     const uint64_t ost[1] = {(uint64_t)p.ldc};
-    int rc = make_tmap_16_sw(tmO, E::kTma, p.out, 2, dims, ost, box, 64);
+    int rc = make_tmap_16(tmO, E::kTma, p.out, 2, dims, ost, box, 64);
     if (rc || !p.residual) return rc;
     const uint64_t rst[1] = {(uint64_t)p.ldr};
-    return make_tmap_16_sw(tmR, E::kTma, p.residual, 2, dims, rst, box, 64);
+    return make_tmap_16(tmR, E::kTma, p.residual, 2, dims, rst, box, 64);
 }
 
+// Picks the tile width once, then builds the W map (W: [N, K] with row stride ldw; its box is one BK x bn tile) and the
+// epilogue's maps for it, and launches.
 template <class E>
-static int run_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmKernelParams& p, cudaStream_t st) {
-    if (p.conv) p.nimg = (int)(p.M / ((long long)p.H * p.W));
+static int run_gemm(const CUtensorMap& tmA, const void* W, long long ldw, GemmKernelParams& p, cudaStream_t st) {
     const int bn = pick_bn(p, g_force_bn);
-    CUtensorMap tmO{}, tmR{};
-    const int rc = make_epilogue_maps<E>(p, bn, &tmO, &tmR);
+    CUtensorMap tmB, tmO{}, tmR{};
+    const uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.N};
+    const uint64_t str[1] = {(uint64_t)ldw};
+    const uint32_t box[2] = {BK, (uint32_t)bn};
+    int rc = make_tmap_16(&tmB, E::kTma, W, 2, dims, str, box);
+    if (rc) return rc;
+    rc = make_epilogue_maps<E>(p, bn, &tmO, &tmR);
     if (rc) return rc;
     if (bn == 256) return launch_gemm<256, E>(tmA, tmB, tmO, tmR, p, st);
     if (bn == 160) return launch_gemm<160, E>(tmA, tmB, tmO, tmR, p, st);
@@ -768,23 +690,13 @@ static int gemm_impl(const char* who, const void* A, long long lda, const void* 
     if (rc) return rc;
     SUPIR_REQUIRE(ldc >= p.n_out, "%s: ldc %lld < output columns %d", who, ldc, p.n_out);
     p.out = out; p.ldc = ldc;
-    const int bn = pick_bn(p, g_force_bn);
-    CUtensorMap tmA, tmB;
-    {
-        const uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
-        const uint64_t str[1] = {(uint64_t)lda};
-        const uint32_t box[2] = {BK, BM};
-        rc = make_tmap_16(&tmA, E::kTma, A, 2, dims, str, box);
-        if (rc) return rc;
-    }
-    {
-        const uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
-        const uint64_t str[1] = {(uint64_t)ldw};
-        const uint32_t box[2] = {BK, (uint32_t)bn};
-        rc = make_tmap_16(&tmB, E::kTma, W, 2, dims, str, box);
-        if (rc) return rc;
-    }
-    return run_gemm<E>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
+    CUtensorMap tmA;
+    const uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
+    const uint64_t str[1] = {(uint64_t)lda};
+    const uint32_t box[2] = {BK, BM};
+    rc = make_tmap_16(&tmA, E::kTma, A, 2, dims, str, box);
+    if (rc) return rc;
+    return run_gemm<E>(tmA, W, ldw, p, reinterpret_cast<cudaStream_t>(stream));
 }
 
 template <class E>
@@ -821,6 +733,7 @@ static int conv_geom_impl(const char* who, const void* x, long long ldx, const v
     p.kchunks = (Cin + BK - 1) / BK;
     p.num_kb = ntaps * p.kchunks;
     p.M = B * H * Wd; p.N = Cout; p.K = ntaps * Cin;
+    p.nimg = B;
     int rc = fill_epilogue(p, ep, Cout);
     if (rc) return rc;
     SUPIR_REQUIRE(ldc >= p.n_out, "%s: ldc %lld < output columns %d", who, ldc, p.n_out);
@@ -828,25 +741,15 @@ static int conv_geom_impl(const char* who, const void* x, long long ldx, const v
     SUPIR_REQUIRE(plain_out || (!p.residual && !p.rowvec), "%s: residual / per-image vector need a plain output layout", who);
     SUPIR_REQUIRE(plain_out || (g.out_sy != 1 || g.out_sx != 1) || (g.out_H == H && g.out_W == Wd), "%s: unit-stride outputs must match the grid", who);
     p.out = out; p.ldc = ldc;
-    const int bn = pick_bn(p, g_force_bn);
-    CUtensorMap tmA, tmB;
-    {
-        // input [B, Hin, Win, Cin]; a tile's box covers TH x TW output pixels = every `stride`-th input pixel (elementStrides)
-        const uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)Win, (uint64_t)Hin, (uint64_t)B};
-        const uint64_t str[3] = {(uint64_t)ldx, (uint64_t)ldx * Win, (uint64_t)ldx * Win * Hin};
-        const uint32_t box[4] = {BK, (uint32_t)(p.TW * g.stride), (uint32_t)(p.TH * g.stride), 1};
-        const uint32_t est[4] = {1, (uint32_t)g.stride, (uint32_t)g.stride, 1};
-        rc = make_tmap_16_strided(&tmA, E::kTma, x, 4, dims, str, box, est);
-        if (rc) return rc;
-    }
-    {
-        const uint64_t dims[2] = {(uint64_t)(ntaps * Cin), (uint64_t)Cout};
-        const uint64_t str[1] = {(uint64_t)(ntaps * Cin)};
-        const uint32_t box[2] = {BK, (uint32_t)bn};
-        rc = make_tmap_16(&tmB, E::kTma, Wp, 2, dims, str, box);
-        if (rc) return rc;
-    }
-    return run_gemm<E>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream));
+    // input [B, Hin, Win, Cin]; a tile's box covers TH x TW output pixels = every `stride`-th input pixel (elementStrides)
+    CUtensorMap tmA;
+    const uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)Win, (uint64_t)Hin, (uint64_t)B};
+    const uint64_t str[3] = {(uint64_t)ldx, (uint64_t)ldx * Win, (uint64_t)ldx * Win * Hin};
+    const uint32_t box[4] = {BK, (uint32_t)(p.TW * g.stride), (uint32_t)(p.TH * g.stride), 1};
+    const uint32_t est[4] = {1, (uint32_t)g.stride, (uint32_t)g.stride, 1};
+    rc = make_tmap_16(&tmA, E::kTma, x, 4, dims, str, box, 128, est);
+    if (rc) return rc;
+    return run_gemm<E>(tmA, Wp, p.K, p, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int supir_gemm_bf16(const void* A, long long lda, const void* W, long long ldw, void* out, long long ldc,

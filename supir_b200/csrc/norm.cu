@@ -10,7 +10,6 @@
 #include "supir_b200.h"
 
 namespace supir {
-int current_device_slot();
 
 // ---------------------------------------------------------------------------------------------
 // GroupNorm statistics: per (image, group) sum and sum of squares in fp64 — deterministic (no floating-point atomics):

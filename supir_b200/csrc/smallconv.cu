@@ -11,7 +11,6 @@
 #include "supir_b200.h"
 
 namespace supir {
-int current_device_slot();
 
 // -------- Cin <= 8 : thread = (pixel, 8 output channels); weights in shared memory as [Cin*9][Cout] --------
 template <class E>

@@ -77,7 +77,7 @@ GEMM_SHAPES = [
 
 
 @pytest.mark.parametrize("shape", GEMM_SHAPES, ids=lambda s: "M%d_N%d_K%d_act%d%s%s" % (s[0], s[1], s[2], s[3], "_b" if s[4] else "", "_r" if s[5] else ""))
-def test_gemm_bench_shapes_all_tiles_and_pair_modes(shape):
+def test_gemm_bench_shapes_all_tiles(shape):
     ops, native = _ops()
     M, N, K, act, with_bias, with_res = shape
     a = _rand((M, K), 11)
