@@ -4,7 +4,8 @@ They let the HOST-side code — weight packing (fused QKV / K|V matrices, GEGLU 
 folding, embedding / context offsets), the module wiring of GLVControl / LightGLVUNet, the VAE step list and its tiled
 executor, the samplers' step logic, unit sharding and exchanges — run without a GPU and be compared with the reference's
 golden outputs, also under gloo with several ranks. The arithmetic of the real kernels is pinned by the -m gpu tests; these
-stand-ins only have to be the same maths (fp32 here, bf16 storage where the kernels store bf16)."""
+stand-ins compute in fp32 and round to the 16-bit type at the points where the kernels round, and
+tests/test_gpu_kernel_edges.py holds them to the kernels' error bounds on the kernels' inputs."""
 import math
 
 import torch
@@ -144,8 +145,8 @@ def groupnorm_apply(x, B, HW, out, gamma, beta, eps, silu, sums=None, mean=None,
 
 def zerosft_apply(h, skip_raw, C1, gamma_beta, out, B, HW, sums, gn_w, gn_b, eps, control_scale, groups=32):
     C = h.shape[1]
-    normed = _bf(_gn(h, B, HW, gn_w, gn_b, eps, groups, sums, None, None))
-    a = normed * (gamma_beta[:, :C].float() + 1.0) + gamma_beta[:, C:].float()
+    normed = _gn(h, B, HW, gn_w, gn_b, eps, groups, sums, None, None)        # fp32: autocast's group_norm returns fp32
+    a = normed * (gamma_beta[:, :C].float() + 1.0).to(out.dtype).float() + gamma_beta[:, C:].float()   # (gamma + 1) is a 16-bit tensor
     h_raw = h.float() if skip_raw is None else torch.cat([h[:, :C1].float(), skip_raw.float()], 1)
     cs = float(control_scale.reshape(-1)[0])
     out.copy_((a * cs + h_raw * (1.0 - cs)).to(out.dtype))
@@ -167,23 +168,24 @@ def layernorm_stats(x, stats, eps=1e-5):
 
 # ---- small convs, data movement, embeddings ----
 def conv3x3_small_cin(x_nchw, w, bias, out, residual=None, w_packed=None, pool=None):
-    y = _nhwc(F.conv2d(_bf(x_nchw), w.float(), None if bias is None else bias.float(), padding=1))
+    y = _nhwc(F.conv2d(x_nchw.to(out.dtype).float(), w.float(), None if bias is None else bias.float(), padding=1))
     if residual is not None:
-        y = _bf(y) + residual.float()
+        y = y.to(out.dtype).float() + residual.float()
     out.copy_(y.to(out.dtype))
     return out
 
 
 def conv3x3_small_cout(x, B, H, W, w, bias, out_nchw, crop=None, packed=None, pool=None):
     wt = w.float().permute(0, 3, 1, 2)                 # [Cout, 3, 3, Cin] -> [Cout, Cin, 3, 3]
-    y = _bf(F.conv2d(_nchw(x, B, H, W), wt, None if bias is None else bias.float(), padding=1))
+    # fp64 sum, one rounding to x's 16-bit type: up to 9 * 512 products per output, and only <= 8 output channels
+    y = F.conv2d(_nchw(x, B, H, W).double(), wt.double(), None if bias is None else bias.double(), padding=1).to(x.dtype).float()
     y0, x0, ch, cw = crop if crop is not None else (0, 0, H, W)
     out_nchw.copy_(y[:, :out_nchw.shape[1], y0:y0 + ch, x0:x0 + cw])
     return out_nchw
 
 
 def conv1x1_small_nchw(x, w, bias, out, in_scale=1.0):
-    out.copy_(F.conv2d(_bf(x * in_scale), w.float()[:, :, None, None], None if bias is None else bias.float()))
+    out.copy_(_bf(F.conv2d(_bf(x * in_scale), w.float()[:, :, None, None], None if bias is None else bias.float())))
     return out
 
 
@@ -197,18 +199,19 @@ def timestep_embedding(t, out):
 
 
 def linear_small_m(x, w, bias, out, silu_in=False, silu_out=False, add=None):
-    xv = _bf(x)
+    r = lambda t: t.to(w.dtype).float()  # noqa: E731  (rounding points in w's 16-bit type)
+    xv = r(x)
     if silu_in:
-        xv = _bf(F.silu(xv))
+        xv = r(F.silu(xv))
     v = xv @ w.float().t()
-    v = _bf(v + (0 if bias is None else bias.float()))
+    v = r(v + (0 if bias is None else bias.float()))
     so = int(silu_out)
     if so & 1:
-        v = _bf(F.silu(v))
+        v = r(F.silu(v))
     if add is not None:
-        v = _bf(v + add)
+        v = r(v + add)
     if so & 2:
-        v = _bf(F.silu(v))
+        v = r(F.silu(v))
     out.copy_(v)
     return out
 
@@ -238,7 +241,7 @@ def copy2d(src, dst):
 
 
 def axpy(a, y, out, scale):
-    out.copy_((a.float() + y.float() * float(scale.reshape(-1)[0])).to(out.dtype))
+    out.copy_((a.float() + (y.float() * float(scale.reshape(-1)[0])).to(out.dtype).float()).to(out.dtype))
     return out
 
 
