@@ -218,21 +218,38 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
                 }
             }
         } else {
-            float ln_rs = 1.f, ln_nm = 0.f;
-            if (p.ln_stats) { const float2 st = __ldg(p.ln_stats + grow); ln_rs = st.x; ln_nm = st.y; }
             constexpr int NJ = BN / 8;
+            float v[NJ][2];
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) { v[j][0] = acc[4 * j + 2 * h]; v[j][1] = acc[4 * j + 2 * h + 1]; }
+            // One branch-free pass per column operand: every load of a pass is issued before the first use, instead of one
+            // load-use round trip per column pair. Columns past N read column N - 1 (their results are never stored).
+            const auto col = [&](int j, int e) { const int n = nt * BN + 8 * j + cq + e; return n < p.N ? n : p.N - 1; };
+            if (p.ln_stats) {
+                const float2 st = __ldg(p.ln_stats + grow);
+#pragma unroll
+                for (int j = 0; j < NJ; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) v[j][e] = fmaf(v[j][e], st.x, -st.y * __ldg(p.ln_colsum + col(j, e)));
+            }
+            if (p.bias) {
+#pragma unroll
+                for (int j = 0; j < NJ; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) v[j][e] += __ldg(p.bias + col(j, e));
+            }
+            if (rv) {
+#pragma unroll
+                for (int j = 0; j < NJ; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) v[j][e] += __ldg(rv + col(j, e));
+            }
 #pragma unroll
             for (int j = 0; j < NJ; ++j) {
                 const int n = nt * BN + 8 * j + cq;
                 if (n >= p.N) break;
                 const bool n1ok = n + 1 < p.N;
-                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-                if (p.ln_stats) {
-                    v0 = fmaf(v0, ln_rs, -ln_nm * __ldg(p.ln_colsum + n));
-                    if (n1ok) v1 = fmaf(v1, ln_rs, -ln_nm * __ldg(p.ln_colsum + n + 1));
-                }
-                if (p.bias) { v0 += __ldg(p.bias + n); if (n1ok) v1 += __ldg(p.bias + n + 1); }
-                if (rv) { v0 += __ldg(rv + n); if (n1ok) v1 += __ldg(rv + n + 1); }
+                float v0 = v[j][0], v1 = v[j][1];
                 if (p.act == 1) { v0 = silu_f(E::round(v0)); v1 = silu_f(E::round(v1)); }
                 if (p.residual) {
                     const float2 rr = E::unpack2(STAGED ? ld_shared_u32(frag + stage_off(r, 8 * j + cq)) : load_res_bits<E>(p, grow, n, n1ok));
@@ -548,14 +565,14 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
 
 // choose the N tile (and with it the schedule, see gemm_pingpong): minimise (tiles per SM) x (per-tile time), with
 //   per-tile time = per_col[bn] * bn * num_kb + overhead[bn]
-// in units of one 160-wide column-k-block. Both terms are fitted to CUDA-event timings of the denoiser step's GEMM / conv shapes
-// at every forced width on an H100 80GB HBM3 at 700 W (1980 MHz): per_col from the K = 5120 residual GEMM (M = 33792,
-// N = 1280), where the mainloop dominates; overhead from the K = 640 residual GEMM (M = 135168, N = 640), where the epilogue
-// and pipeline fill dominate. Under ping-pong (64, 128) the overhead is what the other warpgroup's mainloop does not hide.
-// GEGLU takes the 128-wide ping-pong tile: it was the fastest width on both GEGLU shapes of the step (its epilogue does the
-// most arithmetic per column and hides best under the other warpgroup's mainloop). Re-checked with the staged epilogue by
-// tools/bench_gemm_widths.py on an H100 80GB HBM3 at 400 W (1695-1800 MHz under sw_power_cap): the widths this model picks
-// total 604.3 ms per 34-row denoiser call against 604.2 ms for the fastest width of every shape, so the constants stand.
+// in units of one 160-wide column-k-block. Both terms are a least-squares fit (weighted by launches per call) to
+// tools/bench_gemm_widths.py's per-width timings of every non-GEGLU GEMM / conv signature of a 34-row denoiser call, then
+// adjusted to minimise the total of the widths chosen, on an H100 80GB HBM3 at a 700 W power limit (sw_power_cap). With
+// these constants the chosen widths total 551.0 ms per call against 547.9 ms for the fastest width of every shape (563.9 ms
+// with the constants fitted before the epilogue's operand passes); on a second table from another session, 563.3 against
+// 559.6 ms. Under ping-pong (64, 128) the overhead is what the other warpgroup's mainloop does not hide.
+// GEGLU takes the 128-wide ping-pong tile: its epilogue does the most arithmetic per column and hides best under the other
+// warpgroup's mainloop.
 static int pick_bn(const GemmKernelParams& p, int force_bn) {
     const int m_tiles = p.num_m_tiles, N = p.N, num_kb = p.num_kb;
     if (force_bn == 64 || force_bn == 128 || force_bn == 160 || force_bn == 256) return force_bn;
@@ -569,8 +586,8 @@ static int pick_bn(const GemmKernelParams& p, int force_bn) {
         if (bn > 64 && N <= bn / 2) continue;
         const long long tiles = (long long)m_tiles * ((N + bn - 1) / bn);
         const long long rounds = (tiles + sms - 1) / sms;
-        const double per_col = bn == 256 ? 1.21 : (bn == 160 ? 1.0 : (bn == 128 ? 1.34 : 1.57));
-        const double overhead = bn == 256 ? 7620.0 : (bn == 160 ? 3140.0 : (bn == 128 ? 5460.0 : 1120.0));
+        const double per_col = bn == 256 ? 1.08 : (bn == 160 ? 1.0 : (bn == 128 ? 1.03 : 1.55));
+        const double overhead = bn == 256 ? 2380.0 : (bn == 160 ? 1850.0 : (bn == 128 ? 1430.0 : 780.0));
         const double cost = rounds * (per_col * bn * num_kb + overhead);
         if (cost < best_cost - 1e-9) { best_cost = cost; best = bn; }
     }
@@ -582,9 +599,11 @@ static int g_force_bn = 0;   // supir_set_gemm_tile_n: 0 = pick_bn's choice
 // The staged epilogue needs what TMA can address: a 16-bit output and residual with 16-byte aligned base pointers and row
 // strides (fp32 outputs of the text towers, odd leading dimensions and odd-address residuals take the direct stores), and
 // a whole number of 32-column slabs per tile (not GEGLU at width 160, 80 output columns, which pick_bn never chooses).
+// The output width must end on a 16-byte boundary (n_out % 8 == 0): a TMA store box clipped inside a 16-byte chunk
+// wrote the whole chunk, past the last column, into whatever follows it in the row (a column slice's neighbours).
 static bool can_stage(const GemmKernelParams& p, int bn) {
     const auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-    return !p.out_f32 && (p.act != 2 || bn % 64 == 0) && al16(p.out) && (p.ldc * 2) % 16 == 0 &&
+    return !p.out_f32 && (p.act != 2 || bn % 64 == 0) && p.n_out % 8 == 0 && al16(p.out) && (p.ldc * 2) % 16 == 0 &&
            (!p.residual || (al16(p.residual) && (p.ldr * 2) % 16 == 0));
 }
 
