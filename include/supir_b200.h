@@ -93,7 +93,17 @@ int supir_conv3x3_f16(const void* x, long long ldx, const void* Wp, void* out, l
 int supir_conv_geom_f16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int Hin, int Win, int Cin,
                         int Cout, const supir_conv_geometry* geom, const supir_epilogue* ep, void* stream);
 
-/* debugging / tuning knob: force the N tile (64/128/256), 0 = heuristic */
+/* FP8 linear layers (the transformer blocks' Linears in the `float8_e4m3fn` compute mode): the same kernel with e4m3 operands
+ * (m64nNk32 wgmma) and per-row scales, out[m, n] = epilogue(a_scale[m] * w_scale[n] * sum_k A[m, k] W[n, k]) with fp32
+ * accumulation and the bf16 epilogue of supir_gemm_bf16 after the scale (bias, GEGLU, bf16 rounding points, bf16 residual).
+ * A [M, lda], W [N, ldw]: e4m3 (float8_e4m3fn) codes, 16-byte aligned; K, lda, ldw multiples of 16 (TMA row strides);
+ * a_scale [M], w_scale [N] fp32 (w_scale in the row order of W, e.g. the GEGLU interleave). out is bf16; ep may carry bias,
+ * residual and act 0 / 2 only (no out_f32, ln_stats / ln_colsum, rowvec). Outputs whose width is not a multiple of 8 take
+ * the direct-store epilogue, as in bf16. */
+int supir_gemm_fp8(const void* A, long long lda, const float* a_scale, const void* W, long long ldw, const float* w_scale,
+                   void* out, long long ldc, int M, int N, int K, const supir_epilogue* ep, void* stream);
+
+/* debugging / tuning knob: force the N tile (64/128/160/256), 0 = heuristic (for bf16, fp16 and e4m3 operands) */
 int supir_set_gemm_tile_n(int bn);
 /* ------------------------------------------------------------------------------------------------------------------ */
 /* network entry / exit convolutions with < 8 channels on one side (smallconv.cu)                                     */
@@ -166,6 +176,12 @@ int supir_layernorm_bf16(const void* x, long long ldx, void* y, long long ldy, l
  * pass instead of a read + write pass, and no normalised copy of the activations) */
 int supir_layernorm_stats(const void* x, long long ldx, long long rows, int C, float eps, float* stats, void* stream);
 
+/* LayerNorm of bf16 rows written as e4m3 for supir_gemm_fp8: q [rows, ldq] e4m3 codes and scale [rows] fp32 from the row amax
+ * of the fp32 LayerNorm output (no bf16 rounding in between): scale = amax / 448 (1 for an all-zero row),
+ * q = RNE(y * (448 / amax)). C, ldq multiples of 16, C <= 2048; x, q, gamma, beta 16-byte aligned. */
+int supir_layernorm_quant(const void* x, long long ldx, void* q, long long ldq, float* scale, long long rows, int C,
+                          const float* gamma, const float* beta, float eps, void* stream);
+
 /* fp16 twins of the GroupNorm / ZeroSFT / LayerNorm functions above (fp16 activations, same statistics) */
 int supir_groupnorm_stats_f16(const void* x, long long ldx, int B, int HW, int C, int groups, double* ws, long long ws_doubles,
                               void* stream);
@@ -228,6 +244,9 @@ int supir_nhwc_bf16_to_nchw_f32(const void* x, long long ldx, float* y, int B, i
 int supir_nhwc_bf16_crop_to_nchw_f32(const void* x, long long ldx, float* y, long long ob, long long oc, long long oy, int B,
                                      int H, int W, int C, int crop_y0, int crop_x0, int crop_h, int crop_w, void* stream);
 int supir_f32_to_bf16(const float* x, void* y, long long n, void* stream);
+/* bf16 rows -> e4m3 codes q [rows, ldq] + fp32 scale [rows], the quantization of supir_layernorm_quant (FP8 operand of
+ * supir_gemm_fp8). cols, ldx, ldq multiples of 8; x 16-byte aligned, q 8-byte aligned. */
+int supir_quantize_rows(const void* x, long long ldx, void* q, long long ldq, float* scale, long long rows, int cols, void* stream);
 /* fp16 twins */
 int supir_axpy_f16(const void* a, long long lda, const void* y, long long ldy, void* out, long long ldo, long long rows,
                    int cols, const float* scale, void* stream);

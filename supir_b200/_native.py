@@ -29,6 +29,8 @@ _SIGS = {
     "supir_conv3x3_bf16": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(Epilogue), c_void_p],
     "supir_conv_geom_bf16": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(ConvGeometry),
                              ctypes.POINTER(Epilogue), c_void_p],
+    "supir_gemm_fp8": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, ctypes.POINTER(Epilogue),
+                       c_void_p],
     "supir_set_gemm_tile_n": [c_int],
     "supir_conv3x3_small_cin": [c_void_p, c_ll, c_ll, c_ll, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "supir_im2col_3x3_small_cin": [c_void_p, c_ll, c_ll, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p],
@@ -41,6 +43,7 @@ _SIGS = {
     "supir_zerosft_apply": [c_void_p, c_ll, c_void_p, c_ll, c_int, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p],
     "supir_layernorm_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_int, c_void_p, c_void_p, c_float, c_void_p],
     "supir_layernorm_stats": [c_void_p, c_ll, c_ll, c_int, c_float, c_void_p, c_void_p],
+    "supir_layernorm_quant": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_void_p, c_void_p, c_float, c_void_p],
     "supir_softmax_rows": [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_int, c_float, c_void_p],
     "supir_attention_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p],
     "supir_attention_1head_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_float, c_void_p],
@@ -54,6 +57,7 @@ _SIGS = {
     "supir_nhwc_bf16_to_nchw_f32": [c_void_p, c_ll, c_void_p, c_int, c_int, c_int, c_void_p],
     "supir_nhwc_bf16_crop_to_nchw_f32": [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_ll, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "supir_f32_to_bf16": [c_void_p, c_void_p, c_ll, c_void_p],
+    "supir_quantize_rows": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_void_p],
     "supir_timestep_embedding": [c_void_p, c_void_p, c_int, c_int, c_void_p],
     "supir_linear_small_m": [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p],
     "supir_edm_pre": [c_void_p, c_void_p, c_float, c_float, c_void_p, c_void_p, c_ll, c_void_p],

@@ -4,6 +4,7 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -17,10 +18,12 @@ void count_launch(int n = 1);  // bumps the counter behind supir_launch_count()
 int device_sm_count();
 int current_device_slot();   // cudaGetDevice() clamped to [0, 63]: index of the per-device caches
 
-// Tensor map of 16-bit elements (defined in gemm.cu): dims / strides innermost first, strides in elements; `swizzle` in bytes;
-// `elem_strides` (null: all 1) are TMA traversal strides. Rejects base addresses and strides TMA cannot take.
+// Tensor map of 16-bit elements, or of `elem_bytes`-byte ones (defined in gemm.cu): dims / strides innermost first, strides in
+// elements; `swizzle` in bytes; `elem_strides` (null: all 1) are TMA traversal strides. Rejects base addresses and strides TMA
+// cannot take.
 int make_tmap_16(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
-                 const uint64_t* strides_elems, const uint32_t* box, int swizzle = 128, const uint32_t* elem_strides = nullptr);
+                 const uint64_t* strides_elems, const uint32_t* box, int swizzle = 128, const uint32_t* elem_strides = nullptr,
+                 int elem_bytes = 2);
 
 #define SUPIR_OK 0
 #define SUPIR_ERR_INVALID -1
@@ -99,12 +102,20 @@ __device__ __forceinline__ float2 unpack_f16x2(uint32_t u) {
 //   pack2/unpack2: two fp32 <-> one 32-bit register of two storage values (round to nearest even)
 //   from_f/to_f : scalar conversions; bits: the raw 16 bits
 //   kF16        : selects the wgmma operand types (.f16.f16 instead of .bf16.bf16, see wgmma.cuh)
-//   kTma        : TMA data type of the tensor maps
+//   kTma        : TMA data type of the 16-bit tensor maps (output, residual; and the GEMM operands unless kFp8)
+// GEMM operand side (gemm.cu): the operands are the storage type itself, except under E4m3 below.
+//   kFp8        : e4m3 operands (.e4m3.e4m3, m64nNk32) with per-row / per-column fp32 scales applied in the epilogue
+//   kOpTma      : TMA data type of the operand maps; kOpBytes: bytes per operand element
+//   kBK         : operand elements per k-block = one 128-byte swizzled row (64 16-bit or 128 e4m3 elements)
 // ---------------------------------------------------------------------------------------------
 struct Bf16 {
     using T = __nv_bfloat16;
     static constexpr bool kF16 = false;
     static constexpr CUtensorMapDataType kTma = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    static constexpr bool kFp8 = false;
+    static constexpr CUtensorMapDataType kOpTma = kTma;
+    static constexpr int kOpBytes = 2;
+    static constexpr int kBK = 64;
     static __device__ __forceinline__ float round(float v) { return bf16_round(v); }
     static __device__ __forceinline__ uint32_t pack2(float lo, float hi) { return pack_bf16x2(lo, hi); }
     static __device__ __forceinline__ float2 unpack2(uint32_t u) { return unpack_bf16x2(u); }
@@ -116,6 +127,10 @@ struct F16 {
     using T = __half;
     static constexpr bool kF16 = true;
     static constexpr CUtensorMapDataType kTma = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    static constexpr bool kFp8 = false;
+    static constexpr CUtensorMapDataType kOpTma = kTma;
+    static constexpr int kOpBytes = 2;
+    static constexpr int kBK = 64;
     static __device__ __forceinline__ float round(float v) { return f16_round(v); }
     static __device__ __forceinline__ uint32_t pack2(float lo, float hi) { return pack_f16x2(lo, hi); }
     static __device__ __forceinline__ float2 unpack2(uint32_t u) { return unpack_f16x2(u); }
@@ -123,6 +138,29 @@ struct F16 {
     static __device__ __forceinline__ float to_f(T v) { return __half2float(v); }
     static __device__ __forceinline__ uint32_t bits(T v) { return __half_as_ushort(v); }
 };
+
+// FP8 linear layers (supir_gemm_fp8): e4m3 operands, bf16 storage everywhere else. Every epilogue rounding point is bf16's.
+struct E4m3 : Bf16 {
+    static constexpr bool kFp8 = true;
+    static constexpr CUtensorMapDataType kOpTma = CU_TENSOR_MAP_DATA_TYPE_UINT8;
+    static constexpr int kOpBytes = 1;
+    static constexpr int kBK = 128;
+};
+
+// Row quantization to e4m3 (quantize_rows, LayerNorm-quant): scale = amax / 448 (1 for an all-zero row) and
+// code = RNE(x * (448 / amax)), with the two divisions IEEE-rounded: the codes and scales are those of
+// (x * inv).to(torch.float8_e4m3fn) on the same fp32 values. |x * inv| <= 448 up to one ulp, which rounds to 448: the
+// saturating conversion never saturates a value torch would not round to 448 as well.
+__device__ __forceinline__ void e4m3_row_scale(float amax, float& scale, float& inv) {
+    scale = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+    inv = amax > 0.f ? __fdiv_rn(448.f, amax) : 1.f;
+}
+// four fp32 -> four e4m3 codes in one 32-bit word (first value in the low byte)
+__device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
+    const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3);
+    const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(c, d), __NV_SATFINITE, __NV_E4M3);
+    return (lo & 0xFFFFu) | (hi << 16);
+}
 
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 // erf-form GELU — F.gelu default used by GEGLU (reference sgm/modules/attention.py:91):  gelu(g) = g/2 + |g|/2 * erf(|g|/sqrt2).

@@ -60,6 +60,39 @@ __global__ void copy2d_kernel(const __nv_bfloat16* __restrict__ s, long long lds
     }
 }
 
+// Row quantization to e4m3 for supir_gemm_fp8 (the attention output before to_out, the GEGLU output before ff.net.2): one warp
+// per row, grid-stride over rows; pass 1 takes the row's amax, pass 2 re-reads the row (from L1 / L2) and writes the codes
+// (common.cuh e4m3_row_scale / pack_e4m3x4). cols % 8 == 0.
+__global__ void quantize_rows_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, uint8_t* __restrict__ q, long long ldq,
+                                     float* __restrict__ scale, long long rows, int cols) {
+    const int lane = threadIdx.x & 31;
+    const long long nwarps = (long long)gridDim.x * (blockDim.x >> 5);
+    const int cv = cols >> 3;
+    for (long long r = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); r < rows; r += nwarps) {
+        const __nv_bfloat16* xr = x + r * ldx;
+        float amax = 0.f;
+        for (int c = lane; c < cv; c += 32) {
+            const uint4 u = __ldg(reinterpret_cast<const uint4*>(xr + c * 8));
+            const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {
+                const float2 f = unpack_bf16x2(w[t]);
+                amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+            }
+        }
+        float sc, inv;
+        e4m3_row_scale(warp_max(amax), sc, inv);
+        if (lane == 0) scale[r] = sc;
+        for (int c = lane; c < cv; c += 32) {
+            const uint4 u = __ldg(reinterpret_cast<const uint4*>(xr + c * 8));
+            const float2 f0 = unpack_bf16x2(u.x), f1 = unpack_bf16x2(u.y), f2 = unpack_bf16x2(u.z), f3 = unpack_bf16x2(u.w);
+            const uint32_t lo = pack_e4m3x4(f0.x * inv, f0.y * inv, f1.x * inv, f1.y * inv);
+            const uint32_t hi = pack_e4m3x4(f2.x * inv, f2.y * inv, f3.x * inv, f3.y * inv);
+            __stcs(reinterpret_cast<uint2*>(q + r * ldq + c * 8), make_uint2(lo, hi));
+        }
+    }
+}
+
 // out = a + y * (*scale)   (ZeroCrossAttn: x_in + x * control_scale, SUPIR_v0.py:150); E: 16-bit storage type (common.cuh)
 template <class E>
 __global__ void axpy_kernel(const typename E::T* __restrict__ a, long long lda, const typename E::T* __restrict__ y,
@@ -385,6 +418,19 @@ extern "C" int supir_nhwc_f16_crop_to_nchw_f32(const void* x, long long ldx, flo
                   "supir_nhwc_f16_crop_to_nchw_f32: crop window outside the tile");
     nhwc_crop_to_nchw_f32_kernel<F16><<<blocks_for((long long)B * C * crop_h * crop_w, 256), 256, 0, ST(stream)>>>(
         CH(x), ldx, y, ob, oc, oy, B, H, W, C, crop_y0, crop_x0, crop_h, crop_w);
+    DONE();
+}
+
+extern "C" int supir_quantize_rows(const void* x, long long ldx, void* q, long long ldq, float* scale, long long rows, int cols,
+                                   void* stream) {
+    SUPIR_REQUIRE(x && q && scale, "supir_quantize_rows: null pointer");
+    SUPIR_REQUIRE(rows > 0 && cols > 0 && cols % 8 == 0 && ldx % 8 == 0 && ldq % 8 == 0 && ldx >= cols && ldq >= cols,
+                  "supir_quantize_rows: bad shape rows=%lld cols=%d ldx=%lld ldq=%lld (cols, ldx, ldq multiples of 8)", rows, cols, ldx,
+                  ldq);
+    SUPIR_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q) & 7) == 0 &&
+                  (reinterpret_cast<uintptr_t>(scale) & 3) == 0, "supir_quantize_rows: misaligned pointer (x: 16 bytes, q: 8, scale: 4)");
+    quantize_rows_kernel<<<blocks_for(rows * 32, 256), 256, 0, ST(stream)>>>(CBF(x), ldx, reinterpret_cast<uint8_t*>(q), ldq, scale,
+                                                                             rows, cols);
     DONE();
 }
 

@@ -3,14 +3,15 @@
 //   out[m, n] = epilogue( sum_k A[m, k] * W[n, k] )          E x E -> fp32 (registers) -> E/fp32
 //
 // E is the 16-bit storage type (common.cuh): Bf16 (supir_gemm_bf16 ...) or F16 (the _f16 twins). Every rounding point of
-// the epilogue rounds to E.
+// the epilogue rounds to E. E4m3 (supir_gemm_fp8) is Bf16 storage with e4m3 operands: A and W hold e4m3 codes, and the
+// epilogue first multiplies the accumulator by a_scale[m] * w_scale[n] (per-row scales of both operands).
 //
 // Replaces, on the sampling path of the reference: nn.Linear (sgm/modules/attention.py:213-218,87,106,587,611),
 // nn.Conv2d 1x1 (openaimodel.py:317, SUPIR_v0.py:48,87, model.py:124-126,164-175) and nn.Conv2d 3x3 stride 1 pad 1
 // (openaimodel.py:263,300-307; SUPIR_v0.py:79,82-83; model.py:108-117 ...).
 //
 // Design (one persistent CTA per SM, 384 threads = three warpgroups, warp-specialised):
-//   warpgroup 0, thread 0 : TMA producer.  A tile = 128 rows x 64 k (bf16, 128B-swizzled), W tile = BN rows x 64 k.
+//   warpgroup 0, thread 0 : TMA producer.  A tile = 128 rows x 64 k (bf16; 128 k of e4m3: 128B-swizzled), W tile = BN rows x 64 k.
 //                   GEMM mode: A is a 2-D tensor map over [M, K].
 //                   CONV mode: A is a 4-D tensor map over the NHWC activation [B, H, W, C]; the tile's 128 rows are a
 //                   TH x TW pixel patch and the k-loop runs over (tap, 64-channel chunk); the tap shift is applied to the
@@ -64,6 +65,8 @@ struct GemmKernelParams {
     const float2* ln_stats;  // per-row (rstd, mean * rstd) of A: LayerNorm folded into the epilogue (see supir_epilogue), or null
     const float* ln_colsum;  // [N] row sums of the (gamma-scaled) weight matrix
     int staged;           // 1: the epilogue goes through shared memory and TMA (tmO / tmR); 0: direct global stores
+    const float* a_scale;    // E4m3 only: [M] dequantization scale of each row of A
+    const float* w_scale;    // E4m3 only: [N] dequantization scale of each row of W (accumulator column)
 };
 
 // tile widths 64 and 128 run the ping-pong schedule (each consumer warpgroup owns whole 128 x BN tiles, BN accumulators per
@@ -185,6 +188,8 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
         if (!row.ok) continue;
         const long long grow = row.grow;
         const float* rv = p.rowvec ? p.rowvec + (long long)row.batch * p.rowvec_ld : nullptr;
+        // E4m3: the accumulator times a_scale[row] * w_scale[column] comes first (sa * w_scale[n] below)
+        const float sa = E::kFp8 ? __ldg(p.a_scale + grow) : 1.f;
         if (p.act == 2) {
             // GEGLU: accumulator columns come in groups of 32 = [16 value | 16 gate]; this thread holds value column
             // 8 b + cq (+1) of group g in block 4 g + b and its gate 16 columns later in block 4 g + b + 2
@@ -197,6 +202,10 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
                     const int nv = nt * BN + g * 32 + b * 8 + cq;
                     float xv0 = acc[4 * (4 * g + b) + 2 * h], xv1 = acc[4 * (4 * g + b) + 2 * h + 1];
                     float gv0 = acc[4 * (4 * g + b + 2) + 2 * h], gv1 = acc[4 * (4 * g + b + 2) + 2 * h + 1];
+                    if constexpr (E::kFp8) {
+                        xv0 *= sa * __ldg(p.w_scale + nv); xv1 *= sa * __ldg(p.w_scale + nv + 1);
+                        gv0 *= sa * __ldg(p.w_scale + nv + 16); gv1 *= sa * __ldg(p.w_scale + nv + 17);
+                    }
                     if (p.bias) {
                         xv0 += __ldg(p.bias + nv); xv1 += __ldg(p.bias + nv + 1);
                         gv0 += __ldg(p.bias + nv + 16); gv1 += __ldg(p.bias + nv + 17);
@@ -225,6 +234,12 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
             // One branch-free pass per column operand: every load of a pass is issued before the first use, instead of one
             // load-use round trip per column pair. Columns past N read column N - 1 (their results are never stored).
             const auto col = [&](int j, int e) { const int n = nt * BN + 8 * j + cq + e; return n < p.N ? n : p.N - 1; };
+            if (E::kFp8 && p.w_scale) {     // (a run-time branch, like the passes below: it keeps the passes' loads apart)
+#pragma unroll
+                for (int j = 0; j < NJ; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) v[j][e] *= sa * __ldg(p.w_scale + col(j, e));
+            }
             if (p.ln_stats) {
                 const float2 st = __ldg(p.ln_stats + grow);
 #pragma unroll
@@ -378,8 +393,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                             if (++tx == p.ntaps_x) { tx = 0; ++ty; }
                         }
                     } else {
-                        tma_load_2d(sa, &tmA, &full_bar[stage], kb * BK, mt * BM);
-                        tma_load_2d(sb, &tmB, &full_bar[stage], kb * BK, bn0);
+                        tma_load_2d(sa, &tmA, &full_bar[stage], kb * E::kBK, mt * BM);
+                        tma_load_2d(sb, &tmB, &full_bar[stage], kb * E::kBK, bn0);
                     }
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
@@ -430,7 +445,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 const uint32_t b_addr = smem_u32(smem_b + stage * S::B_BYTES);
                 wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {           // 16 k-elements = 32 bytes inside the 128B swizzle row
+                for (int k = 0; k < 4; ++k) {                 // 32 bytes (16 k-elements, 32 for e4m3) inside the 128B swizzle row
                     const uint64_t db = wgmma_desc_sw128(b_addr + 32 * k);
 #pragma unroll
                     for (int f = 0; f < FRAGS; ++f)
@@ -499,12 +514,12 @@ static PFN_tmapEncodeTiled get_encode_fn() {
     return fn;
 }
 
-// Tensor map of 16-bit elements (bf16 or fp16: `dt`); dims / strides innermost first, strides in ELEMENTS for dims
-// 1..rank-1. `swizzle` in bytes: 128 for GEMM / attention operands, 64 for the staged epilogue's slabs. `elem_strides`
+// Tensor map of 16-bit elements (bf16 or fp16: `dt`), or of `elem_bytes`-byte ones (e4m3 GEMM operands as UINT8); dims /
+// strides innermost first, strides in ELEMENTS for dims 1..rank-1. `swizzle` in bytes: 128 for GEMM / attention operands, 64 for the staged epilogue's slabs. `elem_strides`
 // (null: all 1) are traversal strides: the box spans box[i] tensor elements of dimension i and delivers every
 // elem_strides[i]-th of them, densely packed (a stride-2 convolution's input patch).
 int make_tmap_16(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
-                 const uint64_t* strides_elems, const uint32_t* box, int swizzle, const uint32_t* elem_strides) {
+                 const uint64_t* strides_elems, const uint32_t* box, int swizzle, const uint32_t* elem_strides, int elem_bytes) {
     PFN_tmapEncodeTiled fn = get_encode_fn();
     if (!fn) return set_error(SUPIR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
     cuuint64_t gdim[5], gstr[4];
@@ -514,7 +529,7 @@ int make_tmap_16(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int r
         bx[i] = box[i];
         es[i] = elem_strides ? elem_strides[i] : 1;
     }
-    for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_elems[i] * 2;
+    for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_elems[i] * elem_bytes;
     if ((reinterpret_cast<uintptr_t>(base) & 15) != 0)
         return set_error(SUPIR_ERR_INVALID, "TMA base address %p is not 16-byte aligned", base);
     for (int i = 0; i + 1 < rank; ++i)
@@ -547,7 +562,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
         // (one round: one per SM, two under ping-pong) either share a W tile (m-fastest; A is re-streamed once per n-tile
         // unless it fits L2) or share an A tile (n-fastest; W is re-streamed once per round of m-tiles unless it fits L2)
         const double l2 = 50e6;
-        const double a_bytes = 2.0 * p.M * (p.conv ? p.Cin : p.K), w_bytes = 2.0 * p.N * p.K;
+        const double a_bytes = (double)E::kOpBytes * p.M * (p.conv ? p.Cin : p.K), w_bytes = (double)E::kOpBytes * p.N * p.K;
         const double in_flight = (double)device_sm_count() * (gemm_pingpong(BN) ? 2 : 1);
         const double rounds_m = (double)p.num_m_tiles * p.num_n_tiles / in_flight;
         const double t_mfast = w_bytes + (a_bytes <= l2 ? a_bytes : a_bytes * p.num_n_tiles);
@@ -563,6 +578,11 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
     return SUPIR_OK;
 }
 
+// pick_bn's constants for e4m3 operands, in the order 256, 160, 128, 64. A k-block moves the same 128 bytes per operand row as
+// a 16-bit one, so these start as the bf16 values below; they have not yet been fitted to per-width e4m3 timings.
+static constexpr double FP8_PER_COL[4] = {1.08, 1.0, 1.03, 1.55};
+static constexpr double FP8_OVERHEAD[4] = {2380.0, 1850.0, 1430.0, 780.0};
+
 // choose the N tile (and with it the schedule, see gemm_pingpong): minimise (tiles per SM) x (per-tile time), with
 //   per-tile time = per_col[bn] * bn * num_kb + overhead[bn]
 // in units of one 160-wide column-k-block. Both terms are a least-squares fit (weighted by launches per call) to
@@ -573,6 +593,9 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
 // 559.6 ms. Under ping-pong (64, 128) the overhead is what the other warpgroup's mainloop does not hide.
 // GEGLU takes the 128-wide ping-pong tile: its epilogue does the most arithmetic per column and hides best under the other
 // warpgroup's mainloop.
+// E4m3 (supir_gemm_fp8) has its own constants: a k-block is the same 128 bytes of each operand but twice the k-elements,
+// and the k-loop is half as long for the same K (see fp8 below).
+template <class E>
 static int pick_bn(const GemmKernelParams& p, int force_bn) {
     const int m_tiles = p.num_m_tiles, N = p.N, num_kb = p.num_kb;
     if (force_bn == 64 || force_bn == 128 || force_bn == 160 || force_bn == 256) return force_bn;
@@ -586,8 +609,14 @@ static int pick_bn(const GemmKernelParams& p, int force_bn) {
         if (bn > 64 && N <= bn / 2) continue;
         const long long tiles = (long long)m_tiles * ((N + bn - 1) / bn);
         const long long rounds = (tiles + sms - 1) / sms;
-        const double per_col = bn == 256 ? 1.08 : (bn == 160 ? 1.0 : (bn == 128 ? 1.03 : 1.55));
-        const double overhead = bn == 256 ? 2380.0 : (bn == 160 ? 1850.0 : (bn == 128 ? 1430.0 : 780.0));
+        double per_col, overhead;
+        if constexpr (E::kFp8) {
+            per_col = bn == 256 ? FP8_PER_COL[0] : (bn == 160 ? FP8_PER_COL[1] : (bn == 128 ? FP8_PER_COL[2] : FP8_PER_COL[3]));
+            overhead = bn == 256 ? FP8_OVERHEAD[0] : (bn == 160 ? FP8_OVERHEAD[1] : (bn == 128 ? FP8_OVERHEAD[2] : FP8_OVERHEAD[3]));
+        } else {
+            per_col = bn == 256 ? 1.08 : (bn == 160 ? 1.0 : (bn == 128 ? 1.03 : 1.55));
+            overhead = bn == 256 ? 2380.0 : (bn == 160 ? 1850.0 : (bn == 128 ? 1430.0 : 780.0));
+        }
         const double cost = rounds * (per_col * bn * num_kb + overhead);
         if (cost < best_cost - 1e-9) { best_cost = cost; best = bn; }
     }
@@ -640,12 +669,12 @@ static int make_epilogue_maps(GemmKernelParams& p, int bn, CUtensorMap* tmO, CUt
 // epilogue's maps for it, and launches.
 template <class E>
 static int run_gemm(const CUtensorMap& tmA, const void* W, long long ldw, GemmKernelParams& p, cudaStream_t st) {
-    const int bn = pick_bn(p, g_force_bn);
+    const int bn = pick_bn<E>(p, g_force_bn);
     CUtensorMap tmB, tmO{}, tmR{};
     const uint64_t dims[2] = {(uint64_t)p.K, (uint64_t)p.N};
     const uint64_t str[1] = {(uint64_t)ldw};
-    const uint32_t box[2] = {BK, (uint32_t)bn};
-    int rc = make_tmap_16(&tmB, E::kTma, W, 2, dims, str, box);
+    const uint32_t box[2] = {(uint32_t)E::kBK, (uint32_t)bn};
+    int rc = make_tmap_16(&tmB, E::kOpTma, W, 2, dims, str, box, 128, nullptr, E::kOpBytes);
     if (rc) return rc;
     rc = make_epilogue_maps<E>(p, bn, &tmO, &tmR);
     if (rc) return rc;
@@ -695,7 +724,8 @@ extern "C" int supir_set_gemm_tile_n(int bn) {
 
 template <class E>
 static int gemm_impl(const char* who, const void* A, long long lda, const void* W, long long ldw, void* out, long long ldc, int M,
-                     int N, int K, const supir_epilogue* ep, void* stream) {
+                     int N, int K, const supir_epilogue* ep, void* stream, const float* a_scale = nullptr,
+                     const float* w_scale = nullptr) {
     SUPIR_REQUIRE(A && W && out, "%s: null pointer", who);
     SUPIR_REQUIRE(M > 0 && N > 0 && K > 0, "%s: bad shape M=%d N=%d K=%d", who, M, N, K);
     SUPIR_REQUIRE(lda % 8 == 0 && ldw % 8 == 0, "%s: lda/ldw must be multiples of 8", who);
@@ -703,8 +733,9 @@ static int gemm_impl(const char* who, const void* A, long long lda, const void* 
     GemmKernelParams p{};
     p.M = M; p.N = N; p.K = K;
     p.num_m_tiles = (M + BM - 1) / BM;
-    p.num_kb = (K + BK - 1) / BK;
+    p.num_kb = (K + E::kBK - 1) / E::kBK;
     p.conv = 0;
+    p.a_scale = a_scale; p.w_scale = w_scale;
     int rc = fill_epilogue(p, ep, N);
     if (rc) return rc;
     SUPIR_REQUIRE(ldc >= p.n_out, "%s: ldc %lld < output columns %d", who, ldc, p.n_out);
@@ -712,8 +743,8 @@ static int gemm_impl(const char* who, const void* A, long long lda, const void* 
     CUtensorMap tmA;
     const uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
     const uint64_t str[1] = {(uint64_t)lda};
-    const uint32_t box[2] = {BK, BM};
-    rc = make_tmap_16(&tmA, E::kTma, A, 2, dims, str, box);
+    const uint32_t box[2] = {(uint32_t)E::kBK, BM};
+    rc = make_tmap_16(&tmA, E::kOpTma, A, 2, dims, str, box, 128, nullptr, E::kOpBytes);
     if (rc) return rc;
     return run_gemm<E>(tmA, W, ldw, p, reinterpret_cast<cudaStream_t>(stream));
 }
@@ -779,6 +810,22 @@ extern "C" int supir_gemm_bf16(const void* A, long long lda, const void* W, long
 extern "C" int supir_gemm_f16(const void* A, long long lda, const void* W, long long ldw, void* out, long long ldc,
                               int M, int N, int K, const supir_epilogue* ep, void* stream) {
     return gemm_impl<F16>("supir_gemm_f16", A, lda, W, ldw, out, ldc, M, N, K, ep, stream);
+}
+
+extern "C" int supir_gemm_fp8(const void* A, long long lda, const float* a_scale, const void* W, long long ldw, const float* w_scale,
+                              void* out, long long ldc, int M, int N, int K, const supir_epilogue* ep, void* stream) {
+    const char* who = "supir_gemm_fp8";
+    const auto al = [](const void* q, int b) { return (reinterpret_cast<uintptr_t>(q) & (b - 1)) == 0; };
+    SUPIR_REQUIRE(A && W && out && a_scale && w_scale, "%s: null pointer", who);
+    SUPIR_REQUIRE(K % 16 == 0 && lda % 16 == 0 && ldw % 16 == 0,
+                  "%s: K, lda and ldw must be multiples of 16 (16-byte TMA row strides of e4m3), got K=%d lda=%lld ldw=%lld", who, K,
+                  lda, ldw);
+    SUPIR_REQUIRE(al(A, 16) && al(W, 16), "%s: A and W must be 16-byte aligned", who);
+    SUPIR_REQUIRE(al(a_scale, 4) && al(w_scale, 4), "%s: scales must be 4-byte aligned fp32", who);
+    SUPIR_REQUIRE(al(out, 2) && (!ep || !ep->residual || al(ep->residual, 2)), "%s: out / residual must be 2-byte aligned bf16", who);
+    SUPIR_REQUIRE(!ep || (!ep->out_f32 && !ep->ln_stats && !ep->ln_colsum && !ep->rowvec),
+                  "%s: the FP8 epilogue writes bf16 and takes bias / residual / GEGLU only (no out_f32, ln_stats, rowvec)", who);
+    return gemm_impl<E4m3>(who, A, lda, W, ldw, out, ldc, M, N, K, ep, stream, a_scale, w_scale);
 }
 
 extern "C" int supir_conv_geom_bf16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int Hin, int Win,

@@ -261,11 +261,14 @@ __global__ void sft_apply_kernel(const typename E::T* __restrict__ h, long long 
 
 // ---------------------------------------------------------------------------------------------
 // LayerNorm over the last dim (C <= 2048, C % 8 == 0): one warp per row, row kept in registers.
+// QUANT: the normalised row is written as e4m3 codes qout [rows, ldq] plus a row scale qscale[row] (e4m3_row_scale of the fp32
+// values' amax), for supir_gemm_fp8: no intermediate 16-bit rounding, and y is not written.
 // ---------------------------------------------------------------------------------------------
-template <int MAXV, class E>  // max 16-byte vectors per lane
+template <int MAXV, class E, bool QUANT = false>  // max 16-byte vectors per lane
 __global__ void layernorm_kernel(const typename E::T* __restrict__ x, long long ldx, typename E::T* __restrict__ y,
                                  long long ldy, long long rows, int C, const float* __restrict__ gamma,
-                                 const float* __restrict__ beta, float eps, float2* __restrict__ stats) {
+                                 const float* __restrict__ beta, float eps, float2* __restrict__ stats,
+                                 uint8_t* __restrict__ qout = nullptr, long long ldq = 0, float* __restrict__ qscale = nullptr) {
     const int lane = threadIdx.x & 31;
     const long long nwarps = (long long)gridDim.x * (blockDim.x >> 5);
     long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -316,6 +319,39 @@ __global__ void layernorm_kernel(const typename E::T* __restrict__ x, long long 
         const float rstd = rsqrtf(warp_sum(q) / C + eps);
         if (stats) {                                   // statistics only (LayerNorm folded into the consumer GEMM's epilogue)
             if (lane == 0) stats[row] = make_float2(rstd, mean * rstd);
+            continue;
+        }
+        if constexpr (QUANT) {
+            float amax = 0.f;
+#pragma unroll
+            for (int i = 0; i < MAXV; ++i) {
+                const int vi = lane + i * 32;
+                if (vi < nv) {
+                    const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + vi * 8));
+                    const float4 g1 = __ldg(reinterpret_cast<const float4*>(gamma + vi * 8 + 4));
+                    const float4 b0 = __ldg(reinterpret_cast<const float4*>(beta + vi * 8));
+                    const float4 b1 = __ldg(reinterpret_cast<const float4*>(beta + vi * 8 + 4));
+                    const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+                    const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        v[i][j] = (v[i][j] - mean) * rstd * gg[j] + bb[j];
+                        amax = fmaxf(amax, fabsf(v[i][j]));
+                    }
+                }
+            }
+            float sc, inv;
+            e4m3_row_scale(warp_max(amax), sc, inv);
+            if (lane == 0) qscale[row] = sc;
+#pragma unroll
+            for (int i = 0; i < MAXV; ++i) {
+                const int vi = lane + i * 32;
+                if (vi < nv) {
+                    const uint32_t lo = pack_e4m3x4(v[i][0] * inv, v[i][1] * inv, v[i][2] * inv, v[i][3] * inv);
+                    const uint32_t hi = pack_e4m3x4(v[i][4] * inv, v[i][5] * inv, v[i][6] * inv, v[i][7] * inv);
+                    __stcs(reinterpret_cast<uint2*>(qout + row * ldq + vi * 8), make_uint2(lo, hi));
+                }
+            }
             continue;
         }
 #pragma unroll
@@ -568,9 +604,10 @@ extern "C" int supir_zerosft_apply_f16(const void* h, long long ldh, const void*
                                    sums, gn_weight, gn_bias, eps, control_scale, stream);
 }
 
-template <class E>
+template <class E, bool QUANT = false>
 static int launch_layernorm(const void* x, long long ldx, void* y, long long ldy, long long rows, int C, const float* gamma,
-                            const float* beta, float eps, float2* stats, void* stream);
+                            const float* beta, float eps, float2* stats, void* stream, uint8_t* q = nullptr, long long ldq = 0,
+                            float* qscale = nullptr);
 
 extern "C" int supir_layernorm_stats(const void* x, long long ldx, long long rows, int C, float eps, float* stats, void* stream) {
     SUPIR_REQUIRE(x && stats && rows > 0, "supir_layernorm_stats: bad args");
@@ -600,9 +637,23 @@ extern "C" int supir_layernorm_f16(const void* x, long long ldx, void* y, long l
     return launch_layernorm<F16>(x, ldx, y, ldy, rows, C, gamma, beta, eps, nullptr, stream);
 }
 
-template <class E>
+extern "C" int supir_layernorm_quant(const void* x, long long ldx, void* q, long long ldq, float* scale, long long rows, int C,
+                                     const float* gamma, const float* beta, float eps, void* stream) {
+    SUPIR_REQUIRE(x && q && scale && gamma && beta, "supir_layernorm_quant: null pointer");
+    SUPIR_REQUIRE(rows > 0, "supir_layernorm_quant: bad rows %lld", rows);
+    SUPIR_REQUIRE(C % 16 == 0 && C <= 2048 && ldx % 8 == 0 && ldq % 16 == 0 && ldq >= C && ldx >= C,
+                  "supir_layernorm_quant: unsupported C=%d ldx=%lld ldq=%lld (C, ldq multiples of 16, C <= 2048)", C, ldx, ldq);
+    SUPIR_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(scale) & 3) == 0 && (reinterpret_cast<uintptr_t>(gamma) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(beta) & 15) == 0,
+                  "supir_layernorm_quant: misaligned pointer (x, q, gamma, beta: 16 bytes; scale: 4)");
+    return launch_layernorm<Bf16, true>(x, ldx, nullptr, 0, rows, C, gamma, beta, eps, nullptr, stream,
+                                        reinterpret_cast<uint8_t*>(q), ldq, scale);
+}
+
+template <class E, bool QUANT>
 static int launch_layernorm(const void* x, long long ldx, void* y, long long ldy, long long rows, int C, const float* gamma,
-                            const float* beta, float eps, float2* stats, void* stream) {
+                            const float* beta, float eps, float2* stats, void* stream, uint8_t* q, long long ldq, float* qscale) {
     const int warps = 8;
     long long blocks = (rows + warps - 1) / warps;
     const long long cap = (long long)device_sm_count() * 16;       // a few resident waves; warps then loop over rows
@@ -612,11 +663,11 @@ static int launch_layernorm(const void* x, long long ldx, void* y, long long ldy
     typename E::T* yp = reinterpret_cast<typename E::T*>(y);
     const int nv = C >> 3;
     if (nv <= 96)
-        layernorm_kernel<3, E><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats);
+        layernorm_kernel<3, E, QUANT><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats, q, ldq, qscale);
     else if (nv <= 160)
-        layernorm_kernel<5, E><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats);
+        layernorm_kernel<5, E, QUANT><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats, q, ldq, qscale);
     else
-        layernorm_kernel<8, E><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats);
+        layernorm_kernel<8, E, QUANT><<<(unsigned)blocks, warps * 32, 0, st>>>(xp, ldx, yp, ldy, rows, C, gamma, beta, eps, stats, q, ldq, qscale);
     count_launch();
     SUPIR_CHECK_CUDA(cudaGetLastError());
     return SUPIR_OK;

@@ -1,5 +1,7 @@
-// supir — Hopper warpgroup MMA (wgmma.mma_async) wrappers, 16-bit x 16-bit -> fp32, M = 64 per warpgroup.
-// The operand type follows the element-type traits of common.cuh: E::kF16 selects .f16.f16, otherwise .bf16.bf16.
+// supir — Hopper warpgroup MMA (wgmma.mma_async) wrappers, 16-bit x 16-bit or e4m3 x e4m3 -> fp32, M = 64 per warpgroup.
+// The operand type follows the element-type traits of common.cuh: E::kFp8 selects .e4m3.e4m3 (m64nNk32: 32 one-byte
+// k-elements, the same 32 bytes of each operand row as k16 of 16-bit ones; e4m3 takes no transpose operands),
+// E::kF16 .f16.f16, otherwise .bf16.bf16.
 // Accumulator fragment of m64nNk16 (per thread t of the warpgroup, warp w = t / 32, lane l): element 4 j + e holds
 //   row 16 w + l / 4 + 8 (e >> 1), column 8 j + 2 (l % 4) + (e & 1).
 #pragma once
@@ -25,59 +27,63 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
     return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 
-// D (+)= A[smem] * B[smem]^T, both K-major
-#define SUPIR_WGMMA_SS_N64(TY) \
+// D (+)= A[smem] * B[smem]^T, both K-major (the only layout e4m3 operands support)
+#define SUPIR_WGMMA_SS_N64(KTY, TRANS) \
     asm volatile( \
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t" \
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32" TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n" \
+        "wgmma.mma_async.sync.aligned.m64n64" KTY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1" TRANS ";\n\t}\n" \
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
         : "l"(desc_a), "l"(desc_b), "r"(scale_d))
 template <class E>
 __device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b, int scale_d) {
-    if constexpr (E::kF16) SUPIR_WGMMA_SS_N64(".f16.f16");
-    else SUPIR_WGMMA_SS_N64(".bf16.bf16");
+    if constexpr (E::kFp8) SUPIR_WGMMA_SS_N64("k32.f32.e4m3.e4m3", "");
+    else if constexpr (E::kF16) SUPIR_WGMMA_SS_N64("k16.f32.f16.f16", ", 0, 0");
+    else SUPIR_WGMMA_SS_N64("k16.f32.bf16.bf16", ", 0, 0");
 }
 #undef SUPIR_WGMMA_SS_N64
 
 // D (+)= A[smem] * B[smem]^T, both K-major
-#define SUPIR_WGMMA_SS_N128(TY) \
+#define SUPIR_WGMMA_SS_N128(KTY, TRANS) \
     asm volatile( \
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t" \
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32" TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n" \
+        "wgmma.mma_async.sync.aligned.m64n128" KTY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1" TRANS ";\n\t}\n" \
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
         : "l"(desc_a), "l"(desc_b), "r"(scale_d))
 template <class E>
 __device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, int scale_d) {
-    if constexpr (E::kF16) SUPIR_WGMMA_SS_N128(".f16.f16");
-    else SUPIR_WGMMA_SS_N128(".bf16.bf16");
+    if constexpr (E::kFp8) SUPIR_WGMMA_SS_N128("k32.f32.e4m3.e4m3", "");
+    else if constexpr (E::kF16) SUPIR_WGMMA_SS_N128("k16.f32.f16.f16", ", 0, 0");
+    else SUPIR_WGMMA_SS_N128("k16.f32.bf16.bf16", ", 0, 0");
 }
 #undef SUPIR_WGMMA_SS_N128
 
 // D (+)= A[smem] * B[smem]^T, both K-major
-#define SUPIR_WGMMA_SS_N160(TY) \
+#define SUPIR_WGMMA_SS_N160(KTY, TRANS) \
     asm volatile( \
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\t" \
-        "wgmma.mma_async.sync.aligned.m64n160k16.f32" TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, %80, %81, p, 1, 1, 0, 0;\n\t}\n" \
+        "wgmma.mma_async.sync.aligned.m64n160" KTY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, %80, %81, p, 1, 1" TRANS ";\n\t}\n" \
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]) \
         : "l"(desc_a), "l"(desc_b), "r"(scale_d))
 template <class E>
 __device__ __forceinline__ void wgmma_ss_n160(float (&d)[80], uint64_t desc_a, uint64_t desc_b, int scale_d) {
-    if constexpr (E::kF16) SUPIR_WGMMA_SS_N160(".f16.f16");
-    else SUPIR_WGMMA_SS_N160(".bf16.bf16");
+    if constexpr (E::kFp8) SUPIR_WGMMA_SS_N160("k32.f32.e4m3.e4m3", "");
+    else if constexpr (E::kF16) SUPIR_WGMMA_SS_N160("k16.f32.f16.f16", ", 0, 0");
+    else SUPIR_WGMMA_SS_N160("k16.f32.bf16.bf16", ", 0, 0");
 }
 #undef SUPIR_WGMMA_SS_N160
 
 // D (+)= A[smem] * B[smem]^T, both K-major
-#define SUPIR_WGMMA_SS_N256(TY) \
+#define SUPIR_WGMMA_SS_N256(KTY, TRANS) \
     asm volatile( \
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t" \
-        "wgmma.mma_async.sync.aligned.m64n256k16.f32" TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}\n" \
+        "wgmma.mma_async.sync.aligned.m64n256" KTY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1" TRANS ";\n\t}\n" \
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127]) \
         : "l"(desc_a), "l"(desc_b), "r"(scale_d))
 template <class E>
 __device__ __forceinline__ void wgmma_ss_n256(float (&d)[128], uint64_t desc_a, uint64_t desc_b, int scale_d) {
-    if constexpr (E::kF16) SUPIR_WGMMA_SS_N256(".f16.f16");
-    else SUPIR_WGMMA_SS_N256(".bf16.bf16");
+    if constexpr (E::kFp8) SUPIR_WGMMA_SS_N256("k32.f32.e4m3.e4m3", "");
+    else if constexpr (E::kF16) SUPIR_WGMMA_SS_N256("k16.f32.f16.f16", ", 0, 0");
+    else SUPIR_WGMMA_SS_N256("k16.f32.bf16.bf16", ", 0, 0");
 }
 #undef SUPIR_WGMMA_SS_N256
 

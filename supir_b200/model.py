@@ -45,11 +45,13 @@ class SUPIRModel(nn.Module):
             p.requires_grad = False
         self.first_stage_model.denoise_encoder = copy.deepcopy(self.first_stage_model.encoder)
         self.scale_factor = scale_factor
-        assert ae_dtype in ("fp32", "fp16", "bf16") and diffusion_dtype in ("fp32", "fp16", "bf16")
+        assert ae_dtype in ("fp32", "fp16", "bf16") and diffusion_dtype in ("fp32", "fp16", "bf16", "fp8")
         if ae_dtype == "fp16":
             raise RuntimeError("fp16 cause NaN in AE")
         self.ae_dtype = {"fp32": torch.float32, "bf16": torch.bfloat16}[ae_dtype]
-        self.model.dtype = {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16}[diffusion_dtype]
+        # "fp8": bf16 networks whose transformer-block Linear layers run on e4m3 tensor cores (wrappers.ControlWrapper)
+        self.model.dtype = {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16,
+                            "fp8": torch.float8_e4m3fn}[diffusion_dtype]
         self.p_p, self.n_p = p_p, n_p
         self._shard_group, self._shard = None, False
 

@@ -5,8 +5,9 @@ sgm/modules/diffusionmodules/openaimodel.py:506-961, sgm/modules/attention.py:19
 checkpoints load unchanged — but the torch modules below only OWN parameters. Nothing here runs a torch op on the hot
 path: `pack(dtype)` converts the weights once into the kernel layouts (bf16 or fp16, K-major, fused QKV / KV / GEGLU /
 gamma|beta matrices, fp32 biases) and `run()` issues hand-written sm_90a kernels through the C ABI (supir_b200/ops.py) on
-channels-last activations of that dtype (torch.autocast(bfloat16) or autocast(float16) numerics). Options the SUPIR configs
-never use raise NotImplementedError.
+channels-last activations of that dtype (torch.autocast(bfloat16) or autocast(float16) numerics). `pack(float8_e4m3fn)` is
+the bf16 pack except for the Linear layers inside every BasicTransformerBlock, which hold e4m3 weights with per-row scales and
+run on FP8 tensor cores (see `linear`). Options the SUPIR configs never use raise NotImplementedError.
 """
 import os
 
@@ -82,6 +83,21 @@ def _bias_values(t, dtype):
 
 def _bias_bf16_values(t):
     return _bias_values(t, BF16)
+
+
+def linear(ctx, x, w, out, **kw):
+    """out = epilogue(x @ w^T) for a packed weight `w`: a 16-bit matrix (ops.gemm), or the (e4m3 codes, row scales) pair of an
+    FP8 layer (ops.gemm_fp8), whose input `x` is either such a pair already (layernorm_quant) or a bf16 matrix quantized here
+    (quantize_rows: one extra pass over x)."""
+    if not isinstance(w, tuple):
+        return ops.gemm(x, w, out, **kw)
+    if isinstance(x, tuple):
+        return ops.gemm_fp8(*x, *w, out, **kw)
+    q, sc = ctx.new(x.shape[0], x.shape[1], ops.FP8), ctx.pool.get((x.shape[0],), torch.float32)
+    ops.quantize_rows(x, q, sc)
+    ops.gemm_fp8(q, sc, *w, out, **kw)
+    ctx.pool.put(q, sc)
+    return out
 
 
 def pack_conv3x3(w, dtype=BF16):
@@ -254,8 +270,19 @@ class CrossAttention(nn.Module):
         self.kv_offset = None   # column offset inside Ctx.ctx_kv for text cross-attention
 
     _ln = None      # (gamma, beta) of the LayerNorm in front of the query projection, set by BasicTransformerBlock.pack
+    _fp8 = False    # FP8 query / QKV and output projections, set by BasicTransformerBlock.pack
 
     def pack(self, dtype=BF16):
+        if self._fp8:
+            # e4m3 + per-row scales instead of the bf16 matrices (not kept); the text K|V projection stays bf16
+            if self.is_self:
+                self._wqkv = ops.quantize_weight(torch.cat([self.to_q.weight, self.to_k.weight, self.to_v.weight], 0))
+            else:
+                self._wq = ops.quantize_weight(self.to_q.weight)
+                self._wkv = _bf(torch.cat([self.to_k.weight, self.to_v.weight], 0), dtype)
+            self._c1 = self._bq = None
+            self._wo, self._bo = ops.quantize_weight(self.to_out[0].weight), _bias_values(self.to_out[0].bias, dtype)
+            return
         if self.is_self:
             wqkv = torch.cat([self.to_q.weight, self.to_k.weight, self.to_v.weight], 0)
             if self._ln is not None:
@@ -280,27 +307,27 @@ class CrossAttention(nn.Module):
 
     def run_self(self, ctx, xn, x_res, B, L, stats=None):
         """x_res + to_out(attn(xn)); xn, x_res: [B*L, C]. With a folded LayerNorm xn is the RAW input and `stats` its row
-        statistics (ops.layernorm_stats)."""
+        statistics (ops.layernorm_stats); packed FP8, xn is the (codes, scales) pair of the normalised input (see `linear`)."""
         C = self.inner
         qkv = ctx.new(B * L, 3 * C)
-        ops.gemm(xn, self._wqkv, qkv, **self._ln_args(stats))
+        linear(ctx, xn, self._wqkv, qkv, **self._ln_args(stats))
         a = ctx.new(B * L, C)
         ops.attention(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], a, B, self.heads, L, L)
         ctx.free(qkv)
         out = ctx.new(B * L, x_res.shape[1])
-        ops.gemm(a, self._wo, out, bias=self._bo, residual=x_res)
+        linear(ctx, a, self._wo, out, bias=self._bo, residual=x_res)
         ctx.free(a)
         return out
 
     def run_cross(self, ctx, xn, x_res, B, L, k, v, Lk, residual=True, stats=None):
         C = self.inner
         q = ctx.new(B * L, C)
-        ops.gemm(xn, self._wq, q, **self._ln_args(stats))
+        linear(ctx, xn, self._wq, q, **self._ln_args(stats))
         a = ctx.new(B * L, C)
         ops.attention(q, k, v, a, B, self.heads, L, Lk)
         ctx.free(q)
-        out = ctx.new(B * L, self._wo.shape[0])
-        ops.gemm(a, self._wo, out, bias=self._bo, residual=x_res if residual else None)
+        out = ctx.new(B * L, self.to_out[0].out_features)
+        linear(ctx, a, self._wo, out, bias=self._bo, residual=x_res if residual else None)
         ctx.free(a)
         return out
 
@@ -320,21 +347,25 @@ class FeedForward(nn.Module):
         self.inner = inner
         self.net = nn.Sequential(GEGLU(dim, inner), nn.Dropout(dropout), nn.Linear(inner, dim))
 
+    _fp8 = False    # e4m3 GEGLU and output projections, set by BasicTransformerBlock.pack
+
     def pack(self, dtype=BF16):
         w, b = self.net[0].proj.weight.detach(), self.net[0].proj.bias.detach()
         inner = self.inner
         assert inner % 16 == 0
-        # interleave value / gate rows in groups of 16 so that each 32-column accumulator chunk holds both halves
+        # interleave value / gate rows in groups of 16 so that each 32-column accumulator chunk holds both halves (FP8: each
+        # row keeps its own scale, so the scales follow the same permutation)
         idx = torch.arange(inner, device=w.device).view(-1, 16)
         perm = torch.cat([idx, idx + inner], dim=1).reshape(-1)
-        self._w1, self._b1 = _bf(w[perm], dtype), _bias_values(b[perm], dtype)
-        self._w2, self._b2 = _bf(self.net[2].weight, dtype), _bias_values(self.net[2].bias, dtype)
+        weight = ops.quantize_weight if self._fp8 else (lambda t: _bf(t, dtype))
+        self._w1, self._b1 = weight(w[perm]), _bias_values(b[perm], dtype)
+        self._w2, self._b2 = weight(self.net[2].weight), _bias_values(self.net[2].bias, dtype)
 
     def run(self, ctx, xn, x_res):
-        g = ctx.new(xn.shape[0], self.inner)
-        ops.gemm(xn, self._w1, g, bias=self._b1, act=2)
-        out = ctx.new(xn.shape[0], x_res.shape[1])
-        ops.gemm(g, self._w2, out, bias=self._b2, residual=x_res)
+        g = ctx.new(x_res.shape[0], self.inner)
+        linear(ctx, xn, self._w1, g, bias=self._b1, act=2)
+        out = ctx.new(x_res.shape[0], x_res.shape[1])
+        linear(ctx, g, self._w2, out, bias=self._b2, residual=x_res)
         ctx.free(g)
         return out
 
@@ -351,12 +382,17 @@ class BasicTransformerBlock(nn.Module):
         self.attn2 = CrossAttention(query_dim=dim, context_dim=context_dim, heads=n_heads, dim_head=d_head, dropout=dropout)
         self.norm1, self.norm2, self.norm3 = nn.LayerNorm(dim), nn.LayerNorm(dim), nn.LayerNorm(dim)
 
+    fp8 = False     # set by the network's pack(float8_e4m3fn): the Linear layers below run on e4m3 operands
+
     def pack(self, dtype=BF16):
         for n in (self.norm1, self.norm2, self.norm3):
             pack_norm(n)
         # norm1 -> QKV and norm2 -> to_q are folded into those GEMMs (runs before the children's pack(): modules() yields
         # parents first). norm3 stays a kernel: its consumer is the GEGLU GEMM, whose epilogue is already the bound.
-        self.fuse_ln = FUSE_LN
+        # FP8 folds nothing: the fold would quantize the raw, uncentred rows, whose mean then cancels against mean * colsum
+        # after quantization; each LayerNorm writes its normalised rows as e4m3 instead (layernorm_quant).
+        self.attn1._fp8 = self.attn2._fp8 = self.ff._fp8 = self.fp8
+        self.fuse_ln = FUSE_LN and not self.fp8
         self.attn1._ln = (self.norm1.weight, self.norm1.bias) if self.fuse_ln else None
         self.attn2._ln = (self.norm2.weight, self.norm2.bias) if self.fuse_ln else None
 
@@ -364,6 +400,18 @@ class BasicTransformerBlock(nn.Module):
         C = self.attn2.inner
         off = self.attn2.kv_offset
         k, v = ctx.ctx_kv[:, off:off + C], ctx.ctx_kv[:, off + C:off + 2 * C]
+        if self.fp8:
+            nq = (ctx.new(x.shape[0], x.shape[1], ops.FP8), ctx.pool.get((x.shape[0],), torch.float32))
+            ops.layernorm_quant(x, self.norm1._w, self.norm1._b, *nq, self.norm1.eps)
+            x1 = self.attn1.run_self(ctx, nq, x, B, L)
+            ctx.free(x)
+            ops.layernorm_quant(x1, self.norm2._w, self.norm2._b, *nq, self.norm2.eps)
+            x2 = self.attn2.run_cross(ctx, nq, x1, B, L, k, v, ctx.Lctx)
+            ctx.free(x1)
+            ops.layernorm_quant(x2, self.norm3._w, self.norm3._b, *nq, self.norm3.eps)
+            x3 = self.ff.run(ctx, nq, x2)
+            ctx.free(x2, *nq)
+            return x3
         n = ctx.new(*x.shape)
         if self.fuse_ln:
             st = ctx.pool.get((x.shape[0], 2), torch.float32)
@@ -558,15 +606,21 @@ class _UNetBase(nn.Module):
     # ---- packing -----------------------------------------------------------------------------------------------------
     def pack(self, dtype=BF16):
         """Convert parameters into kernel layouts (call again after load_state_dict / .to()). `dtype` is the compute dtype:
-        torch.bfloat16, or torch.float16 for the fp16 mode (every 16-bit weight, bias value and activation in fp16)."""
-        if dtype not in (BF16, ops.F16):
-            raise ValueError(f"compute dtype {dtype} is not supported (bfloat16 or float16)")
+        torch.bfloat16, or torch.float16 for the fp16 mode (every 16-bit weight, bias value and activation in fp16), or
+        torch.float8_e4m3fn for the FP8 mode: bf16 everywhere except the Linear layers of every BasicTransformerBlock (QKV,
+        to_out, the cross-attention's to_q, GEGLU, ff.net.2), which hold e4m3 weights with one fp32 scale per output channel
+        and take e4m3 activations with one scale per row."""
+        if dtype not in (BF16, ops.F16, ops.FP8):
+            raise ValueError(f"compute dtype {dtype} is not supported (bfloat16, float16 or float8_e4m3fn)")
+        fp8 = dtype == ops.FP8
+        dtype = BF16 if fp8 else dtype
         res, xattn = [], []
         for m in self.modules():
             if isinstance(m, ResBlock):
                 res.append(m)
             if isinstance(m, BasicTransformerBlock):
                 xattn.append(m.attn2)
+                m.fp8 = fp8
         off = 0
         for r in res:
             r.emb_offset = off
@@ -590,6 +644,7 @@ class _UNetBase(nn.Module):
                     _bias_values(le[2].bias, dtype))
         self._packed_device = self._emb_w.device
         self._packed_dtype = dtype
+        self._fp8_linears = fp8
         return self
 
     def project_context(self, context_16, out):
@@ -700,6 +755,7 @@ class LightGLVUNet(_UNetBase):
 
     def pack(self, dtype=BF16):
         super().pack(dtype)
+        dtype = self._packed_dtype
         pack_norm(self.out[0])
         w = self.out[2].weight.detach()
         self._wout = w.to(dtype).to(torch.float32).permute(0, 2, 3, 1).contiguous()     # [Cout, 3, 3, Cin]

@@ -6,6 +6,9 @@ dimension handed to the kernels (column slices of wider buffers are fine).
 
 The ops the diffusion networks use also take fp16 operands (their fp16 compute mode): each picks the bf16 entry point or its
 `_f16` twin from the dtype of its 16-bit operands, and refuses operands that mix the two before anything is launched.
+
+FP8 linear layers (the networks' float8_e4m3fn mode): gemm_fp8 multiplies e4m3 operands with one fp32 scale per row of each
+(quantize_weight at pack time; quantize_rows / layernorm_quant for the activations) into a bf16 result.
 """
 import ctypes
 
@@ -22,6 +25,8 @@ CONV_GEOM = os.environ.get("SUPIR_B200_CONV_GEOM", "1") != "0"
 
 BF16 = torch.bfloat16
 F16 = torch.float16
+FP8 = torch.float8_e4m3fn
+E4M3_MAX = 448.0
 
 
 def call(name, *args):
@@ -135,6 +140,60 @@ def gemm(a, w, out, bias=None, rowvec=None, rows_per_batch=0, residual=None, act
     call(name, _ptr(a), a.stride(0), _ptr(w), w.stride(0), _ptr(out), out.stride(0), M, N, K,
          ctypes.byref(ep), _stream())
     return out
+
+
+def e4m3_row_scales(x):
+    """(scale, inverse) per row of an fp32 matrix, the quantization of every FP8 operand: scale = amax / 448 and
+    inverse = 448 / amax (both 1 for an all-zero row); codes = (x * inverse).to(float8_e4m3fn)."""
+    amax = x.abs().amax(dim=1)
+    pos = amax > 0
+    one, fmax = torch.ones_like(amax), torch.full_like(amax, E4M3_MAX)
+    # tensor / tensor: IEEE-rounded divisions, as in the kernels (torch divides by a Python scalar as a product with its
+    # reciprocal, which rounds twice)
+    return torch.where(pos, amax / fmax, one), torch.where(pos, fmax / torch.where(pos, amax, one), one)
+
+
+def quantize_weight(w):
+    """Pack-time FP8 weight: (e4m3 codes [N, K], fp32 scale [N]), one scale per output channel (row) of the bf16 matrix the
+    bf16 pack would use."""
+    wf = w.detach().to(BF16).to(torch.float32)
+    scale, inv = e4m3_row_scales(wf)
+    return (wf * inv[:, None]).to(FP8).contiguous(), scale.contiguous()
+
+
+def gemm_fp8(a_q, a_scale, w_q, w_scale, out, bias=None, residual=None, act=0, ln=None):
+    """out[M, N'] = epilogue(a_scale[m] * w_scale[n] * (a_q[M, K] @ w_q[N, K]^T)) (supir_gemm_fp8): e4m3 operands, fp32 row
+    scales, bf16 `out` / `residual`; N' = N/2 for act=2 (GEGLU). There is no folded LayerNorm: quantize the normalised rows
+    with layernorm_quant instead."""
+    if ln is not None:
+        raise ValueError("gemm_fp8: no folded LayerNorm (ln=); quantize the normalised activations with layernorm_quant")
+    if a_q.dtype != FP8 or w_q.dtype != FP8:
+        raise TypeError(f"gemm_fp8: operands must both be float8_e4m3fn (got {a_q.dtype}, {w_q.dtype})")
+    if out.dtype != BF16 or (residual is not None and residual.dtype != BF16):
+        raise TypeError("gemm_fp8: out and residual are bfloat16")
+    if a_scale.dtype != torch.float32 or w_scale.dtype != torch.float32:
+        raise TypeError("gemm_fp8: scales are float32")
+    _need_cuda(a_q, a_scale, w_q, w_scale, out)
+    _mat(a_q, FP8), _mat(w_q, FP8)
+    M, K = a_q.shape
+    N = w_q.shape[0]
+    assert w_q.shape[1] == K and out.shape[0] == M and out.shape[1] == (N // 2 if act == 2 else N), (a_q.shape, w_q.shape, out.shape)
+    assert a_scale.shape == (M,) and w_scale.shape == (N,) and a_scale.is_contiguous() and w_scale.is_contiguous()
+    ep = _epilogue(bias, None, 0, residual, act, False)
+    call("supir_gemm_fp8", _ptr(a_q), a_q.stride(0), _ptr(a_scale), _ptr(w_q), w_q.stride(0), _ptr(w_scale), _ptr(out), out.stride(0),
+         M, N, K, ctypes.byref(ep), _stream())
+    return out
+
+
+def quantize_rows(x, q, scale):
+    """Row quantization of a bf16 matrix for gemm_fp8: q (e4m3, x's shape) and scale (fp32 [rows]) per e4m3_row_scales."""
+    if x.dtype != BF16 or q.dtype != FP8 or scale.dtype != torch.float32:
+        raise TypeError(f"quantize_rows: bfloat16 -> float8_e4m3fn + float32 (got {x.dtype}, {q.dtype}, {scale.dtype})")
+    _need_cuda(x, q, scale)
+    _mat(x), _mat(q, FP8)
+    assert q.shape == x.shape and scale.shape == (x.shape[0],) and scale.is_contiguous()
+    call("supir_quantize_rows", _ptr(x), x.stride(0), _ptr(q), q.stride(0), _ptr(scale), x.shape[0], x.shape[1], _stream())
+    return q, scale
 
 
 def conv3x3(x, B, H, W, wp, out, bias=None, rowvec=None, residual=None, act=0):
@@ -286,6 +345,19 @@ def layernorm(x, out, gamma, beta, eps=1e-5):
     call(name, _ptr(x), x.stride(0), _ptr(out), out.stride(0), x.shape[0], x.shape[1], _ptr(gamma),
          _ptr(beta), float(eps), _stream())
     return out
+
+
+def layernorm_quant(x, gamma, beta, q, scale, eps=1e-5):
+    """LayerNorm of bf16 rows x written as gemm_fp8's operand: q (e4m3, x's shape) and scale (fp32 [rows]) quantized per
+    e4m3_row_scales from the fp32 normalised values (no bf16 rounding in between)."""
+    if x.dtype != BF16 or q.dtype != FP8 or scale.dtype != torch.float32:
+        raise TypeError(f"layernorm_quant: bfloat16 -> float8_e4m3fn + float32 (got {x.dtype}, {q.dtype}, {scale.dtype})")
+    _need_cuda(x, q, scale)
+    _mat(x), _mat(q, FP8)
+    assert q.shape == x.shape and scale.shape == (x.shape[0],) and scale.is_contiguous()
+    call("supir_layernorm_quant", _ptr(x), x.stride(0), _ptr(q), q.stride(0), _ptr(scale), x.shape[0], x.shape[1], _ptr(gamma),
+         _ptr(beta), float(eps), _stream())
+    return q, scale
 
 
 def layernorm_stats(x, stats, eps=1e-5):

@@ -65,7 +65,7 @@ def load_QF_ckpt(config_path):
 
 def convert_dtype(dtype_str):
     try:
-        return {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16}[dtype_str]
+        return {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16, "fp8": torch.float8_e4m3fn}[dtype_str]
     except KeyError:
         raise NotImplementedError(dtype_str) from None
 

@@ -6,7 +6,8 @@ but one call is one CUDA-graph replay: GLVControl + LightGLVUNet are captured on
 static input/output buffers, so the ~2000 kernel launches of a denoiser call cost no Python or launch-API time.
 
 `.dtype` selects the compute dtype of both networks: torch.float16 runs them in fp16 (torch.autocast(float16) numerics, the
-reference's default `diffusion_dtype`), torch.bfloat16 in bf16; any other value (fp32) warns and computes bf16.
+reference's default `diffusion_dtype`), torch.bfloat16 in bf16, torch.float8_e4m3fn in bf16 with the transformer blocks'
+Linear layers on FP8 tensor cores (nets.py); any other value (fp32) warns and computes bf16.
 """
 import os
 import warnings
@@ -95,19 +96,26 @@ class ControlWrapper(nn.Module):
 
     @staticmethod
     def _compute_dtype(dtype):
+        """dtype of the activations, plans and pools: fp16 or bf16 (also in the FP8 mode)."""
         return torch.float16 if dtype == torch.float16 else torch.bfloat16
+
+    @classmethod
+    def _pack_mode(cls, dtype):
+        """What the networks are packed for (nets._UNetBase.pack): the compute dtype, or float8_e4m3fn for the FP8 linears."""
+        return ops.FP8 if dtype == ops.FP8 else cls._compute_dtype(dtype)
 
     @property
     def dtype(self):
-        """The requested dtype (`diffusion_dtype`): float16 computes in fp16, anything else in bf16."""
+        """The requested dtype (`diffusion_dtype`): float16 computes in fp16, float8_e4m3fn in bf16 with FP8 transformer
+        linears, anything else in bf16."""
         return self._dtype
 
     @dtype.setter
     def dtype(self, value):
         old = getattr(self, "_dtype", None)
         self._dtype = value
-        if old is not None and self._compute_dtype(old) != self._compute_dtype(value):
-            self.invalidate()           # packed weights and captured graphs are in the old compute dtype: drop them
+        if old is not None and self._pack_mode(old) != self._pack_mode(value):
+            self.invalidate()           # packed weights and captured graphs are in the old mode: drop them
 
     @property
     def compute_dtype(self):
@@ -132,8 +140,8 @@ class ControlWrapper(nn.Module):
         return r
 
     def pack(self):
-        self.diffusion_model.pack(self.compute_dtype)
-        self.control_model.pack(self.compute_dtype)
+        self.diffusion_model.pack(self._pack_mode(self._dtype))
+        self.control_model.pack(self._pack_mode(self._dtype))
         self._packed = True
         return self
 
@@ -147,8 +155,8 @@ class ControlWrapper(nn.Module):
             raise RuntimeError("ControlWrapper.forward called before load_control_model()")
         if not x.is_cuda:
             raise RuntimeError("supir_b200.ControlWrapper needs CUDA tensors: the backend has no CPU path")
-        if self.dtype not in (torch.bfloat16, torch.float16) and not self._warned:
-            warnings.warn(f"supir_b200 computes the diffusion networks in bf16 or fp16; dtype {self.dtype} computes in bf16")
+        if self.dtype not in (torch.bfloat16, torch.float16, ops.FP8) and not self._warned:
+            warnings.warn(f"supir_b200 computes the diffusion networks in bf16, fp16 or fp8; dtype {self.dtype} computes in bf16")
             self._warned = True
         if not self._packed:
             self.pack()

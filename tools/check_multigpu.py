@@ -1,6 +1,6 @@
-"""torchrun --nproc-per-node N tools/check_multigpu.py [--dtype bf16|fp16] : the unit-sharded tiled sampler and the tile-sharded
+"""torchrun --nproc-per-node N tools/check_multigpu.py [--dtype bf16|fp16|fp8] : the unit-sharded tiled sampler and the tile-sharded
 VAE give the same result as the single-GPU path, bit for bit, on every rank (also run by tests/test_gpu_multigpu.py and, with
---dtype fp16, by tests/test_gpu_fp16.py when >= 2 GPUs). --dtype is the compute dtype of the diffusion networks."""
+--dtype fp16 / fp8, by tests/test_gpu_fp16.py / test_gpu_fp8.py when >= 2 GPUs). --dtype is the compute dtype of the diffusion networks."""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -21,7 +21,7 @@ def main():
         unet = nets.LightGLVUNet(mode="XL-base", project_type="ZeroSFT", project_channel_scale=2, **cfg)
         ctrl = nets.GLVControl(input_upscale=1, **cfg)
     dname = sys.argv[sys.argv.index("--dtype") + 1] if "--dtype" in sys.argv else "bf16"
-    net = wrappers.ControlWrapper(unet, dtype={"bf16": torch.bfloat16, "fp16": torch.float16}[dname])
+    net = wrappers.ControlWrapper(unet, dtype={"bf16": torch.bfloat16, "fp16": torch.float16, "fp8": torch.float8_e4m3fn}[dname])
     net.load_control_model(ctrl)
     net.to_empty(device="cuda")
     net.load_state_dict(sd)
