@@ -102,6 +102,15 @@ int supir_conv_geom_f16(const void* x, long long ldx, const void* Wp, void* out,
  * the direct-store epilogue, as in bf16. */
 int supir_gemm_fp8(const void* A, long long lda, const float* a_scale, const void* W, long long ldw, const float* w_scale,
                    void* out, long long ldc, int M, int N, int K, const supir_epilogue* ep, void* stream);
+/* FP8 3x3 convolutions (the ResBlocks' in_layers.2 / out_layers.3 in the FP8 convs mode): supir_conv3x3_bf16's implicit GEMM
+ * (stride 1, pad 1, plain output layout) on e4m3 operands, 128-channel k-blocks. x [B*H*W, ldx] e4m3 NHWC codes with one fp32
+ * scale per image, x_scale [B]; Wp [Cout, 9*Cin] e4m3 codes in supir_conv3x3_bf16's (kh, kw, cin) order with one fp32 scale
+ * per output channel, w_scale [Cout]. out[p, n] = epilogue(x_scale[image of p] * w_scale[n] * sum_k x[.] Wp[n, k]), then the
+ * bf16 epilogue of supir_conv3x3_bf16: bias, rowvec (per-image vector), SiLU, residual; out / residual bf16, no out_f32,
+ * ln_stats or GEGLU. Cin, ldx multiples of 16; x, Wp 16-byte aligned. Cin need not be a multiple of 128: the last chunk of
+ * each tap reads TMA's zero fill past Cin. */
+int supir_conv3x3_fp8(const void* x, long long ldx, const float* x_scale, const void* Wp, const float* w_scale, void* out,
+                      long long ldc, int B, int H, int W, int Cin, int Cout, const supir_epilogue* ep, void* stream);
 
 /* debugging / tuning knob: force the N tile (64/128/160/256), 0 = heuristic (for bf16, fp16 and e4m3 operands) */
 int supir_set_gemm_tile_n(int bn);
@@ -181,6 +190,14 @@ int supir_layernorm_stats(const void* x, long long ldx, long long rows, int C, f
  * q = RNE(y * (448 / amax)). C, ldq multiples of 16, C <= 2048; x, q, gamma, beta 16-byte aligned. */
 int supir_layernorm_quant(const void* x, long long ldx, void* q, long long ldq, float* scale, long long rows, int C,
                           const float* gamma, const float* beta, float eps, void* stream);
+/* GroupNorm [+ SiLU] of bf16 x [B, HW, ldx] written as e4m3 for supir_conv3x3_fp8: q [B*HW, ldq] codes and scale [B] fp32,
+ * one per image, from the amax of the image's fp32 apply values (those supir_groupnorm_apply computes, no bf16 rounding in
+ * between): scale = amax / 448 (1 for an all-zero image), q = RNE(y * (448 / amax)). Statistics from `sums` of
+ * supir_groupnorm_stats. amax_ws [B] is scratch for the per-image maximum, reset on `stream` by this call (two kernels: a
+ * read-only amax pass, then the apply-quant pass). C, ldq multiples of 16, ldx of 8; x, q 16-byte aligned. */
+int supir_groupnorm_apply_quant(const void* x, long long ldx, void* q, long long ldq, float* scale, unsigned int* amax_ws, int B,
+                                int HW, int C, int groups, const double* sums, const float* gamma, const float* beta, float eps,
+                                int silu, void* stream);
 
 /* fp16 twins of the GroupNorm / ZeroSFT / LayerNorm functions above (fp16 activations, same statistics) */
 int supir_groupnorm_stats_f16(const void* x, long long ldx, int B, int HW, int C, int groups, double* ws, long long ws_doubles,

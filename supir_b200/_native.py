@@ -31,6 +31,8 @@ _SIGS = {
                              ctypes.POINTER(Epilogue), c_void_p],
     "supir_gemm_fp8": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, ctypes.POINTER(Epilogue),
                        c_void_p],
+    "supir_conv3x3_fp8": [c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int,
+                          ctypes.POINTER(Epilogue), c_void_p],
     "supir_set_gemm_tile_n": [c_int],
     "supir_conv3x3_small_cin": [c_void_p, c_ll, c_ll, c_ll, c_void_p, c_void_p, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "supir_im2col_3x3_small_cin": [c_void_p, c_ll, c_ll, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p],
@@ -44,6 +46,8 @@ _SIGS = {
     "supir_layernorm_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_int, c_void_p, c_void_p, c_float, c_void_p],
     "supir_layernorm_stats": [c_void_p, c_ll, c_ll, c_int, c_float, c_void_p, c_void_p],
     "supir_layernorm_quant": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_void_p, c_void_p, c_float, c_void_p],
+    "supir_groupnorm_apply_quant": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                    c_void_p, c_float, c_int, c_void_p],
     "supir_softmax_rows": [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_int, c_float, c_void_p],
     "supir_attention_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p],
     "supir_attention_1head_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_float, c_void_p],

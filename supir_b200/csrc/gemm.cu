@@ -3,8 +3,9 @@
 //   out[m, n] = epilogue( sum_k A[m, k] * W[n, k] )          E x E -> fp32 (registers) -> E/fp32
 //
 // E is the 16-bit storage type (common.cuh): Bf16 (supir_gemm_bf16 ...) or F16 (the _f16 twins). Every rounding point of
-// the epilogue rounds to E. E4m3 (supir_gemm_fp8) is Bf16 storage with e4m3 operands: A and W hold e4m3 codes, and the
-// epilogue first multiplies the accumulator by a_scale[m] * w_scale[n] (per-row scales of both operands).
+// the epilogue rounds to E. E4m3 (supir_gemm_fp8, supir_conv3x3_fp8) is Bf16 storage with e4m3 operands: A and W hold e4m3
+// codes, and the epilogue first multiplies the accumulator by a_scale[m] * w_scale[n] (per-row scales of both operands; in conv
+// mode a_scale is per image, a_scale[image of m]).
 //
 // Replaces, on the sampling path of the reference: nn.Linear (sgm/modules/attention.py:213-218,87,106,587,611),
 // nn.Conv2d 1x1 (openaimodel.py:317, SUPIR_v0.py:48,87, model.py:124-126,164-175) and nn.Conv2d 3x3 stride 1 pad 1
@@ -14,7 +15,7 @@
 //   warpgroup 0, thread 0 : TMA producer.  A tile = 128 rows x 64 k (bf16; 128 k of e4m3: 128B-swizzled), W tile = BN rows x 64 k.
 //                   GEMM mode: A is a 2-D tensor map over [M, K].
 //                   CONV mode: A is a 4-D tensor map over the NHWC activation [B, H, W, C]; the tile's 128 rows are a
-//                   TH x TW pixel patch and the k-loop runs over (tap, 64-channel chunk); the tap shift is applied to the
+//                   TH x TW pixel patch and the k-loop runs over (tap, BK-channel chunk); the tap shift is applied to the
 //                   TMA coordinates, and TMA's out-of-bounds zero fill IS the conv padding (no im2col buffer).
 //   warpgroups 1, 2       : wgmma consumers (m64nBNk16, fp32 accumulators in registers, one wgmma group kept in flight).
 //                   BN in {160, 256}, cooperative: rows [0, 64) and [64, 128) of every tile. BN in {64, 128}, ping-pong: each
@@ -65,7 +66,7 @@ struct GemmKernelParams {
     const float2* ln_stats;  // per-row (rstd, mean * rstd) of A: LayerNorm folded into the epilogue (see supir_epilogue), or null
     const float* ln_colsum;  // [N] row sums of the (gamma-scaled) weight matrix
     int staged;           // 1: the epilogue goes through shared memory and TMA (tmO / tmR); 0: direct global stores
-    const float* a_scale;    // E4m3 only: [M] dequantization scale of each row of A
+    const float* a_scale;    // E4m3 only: [M] dequantization scale of each row of A (conv mode: [nimg], one per image)
     const float* w_scale;    // E4m3 only: [N] dequantization scale of each row of W (accumulator column)
 };
 
@@ -188,8 +189,9 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
         if (!row.ok) continue;
         const long long grow = row.grow;
         const float* rv = p.rowvec ? p.rowvec + (long long)row.batch * p.rowvec_ld : nullptr;
-        // E4m3: the accumulator times a_scale[row] * w_scale[column] comes first (sa * w_scale[n] below)
-        const float sa = E::kFp8 ? __ldg(p.a_scale + grow) : 1.f;
+        // E4m3: the accumulator times a_scale[row] * w_scale[column] comes first (sa * w_scale[n] below); a convolution's
+        // activation scale is per image (a pixel's k-sum spans 9 input pixels: only a scale they share factors out of it)
+        const float sa = E::kFp8 ? __ldg(p.a_scale + (p.conv ? (long long)row.batch : grow)) : 1.f;
         if (p.act == 2) {
             // GEGLU: accumulator columns come in groups of 32 = [16 value | 16 gate]; this thread holds value column
             // 8 b + cq (+1) of group g in block 4 g + b and its gate 16 columns later in block 4 g + b + 2
@@ -376,7 +378,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 int b = 0, y0 = 0, x0 = 0;
                 if (p.conv) conv_pixel(p, mt, 0, b, y0, x0);
                 const int bn0 = nt * BN;
-                // conv mode walks (tap row, tap column, 64-channel chunk) with counters: no division in the per-k-block path
+                // conv mode walks (tap row, tap column, BK-channel chunk) with counters: no division in the per-k-block path
                 int cc = 0, tx = 0, ty = 0, wcol = 0;
                 const int ax0 = x0 * p.stride + p.off_x, ay0 = y0 * p.stride + p.off_y;
                 for (int kb = 0; kb < p.num_kb; ++kb) {
@@ -385,8 +387,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     uint8_t* sa = smem_a + stage * S::A_BYTES;
                     uint8_t* sb = smem_b + stage * S::B_BYTES;
                     if (p.conv) {
-                        tma_load_4d(sa, &tmA, &full_bar[stage], cc * BK, ax0 + tx, ay0 + ty, b);
-                        tma_load_2d(sb, &tmB, &full_bar[stage], wcol + cc * BK, bn0);
+                        tma_load_4d(sa, &tmA, &full_bar[stage], cc * E::kBK, ax0 + tx, ay0 + ty, b);
+                        tma_load_2d(sb, &tmB, &full_bar[stage], wcol + cc * E::kBK, bn0);
                         if (++cc == p.kchunks) {                       // next tap: W columns advance by Cin
                             cc = 0;
                             wcol += p.Cin;
@@ -749,9 +751,12 @@ static int gemm_impl(const char* who, const void* A, long long lda, const void* 
     return run_gemm<E>(tmA, W, ldw, p, reinterpret_cast<cudaStream_t>(stream));
 }
 
+// E4m3: x and Wp hold e4m3 codes, with a_scale [B] (one per image) and w_scale [Cout]. Channel counts that are not a multiple
+// of E::kBK read TMA's zero fill past Cin in the last chunk of every tap (its W columns are the next tap's: zero times them).
 template <class E>
 static int conv_geom_impl(const char* who, const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int Hin, int Win,
-                          int Cin, int Cout, const supir_conv_geometry& g, const supir_epilogue* ep, void* stream) {
+                          int Cin, int Cout, const supir_conv_geometry& g, const supir_epilogue* ep, void* stream,
+                          const float* a_scale = nullptr, const float* w_scale = nullptr) {
     SUPIR_REQUIRE(x && Wp && out, "%s: null pointer", who);
     SUPIR_REQUIRE(B > 0 && Hin > 0 && Win > 0 && Cin > 0 && Cout > 0, "%s: bad shape", who);
     SUPIR_REQUIRE(Cin % 8 == 0 && ldx % 8 == 0 && ldx >= Cin, "%s: Cin/ldx must be multiples of 8", who);
@@ -780,10 +785,11 @@ static int conv_geom_impl(const char* who, const void* x, long long ldx, const v
     p.tiles_x = (Wd + p.TW - 1) / p.TW;
     p.tiles_y = (H + p.TH - 1) / p.TH;
     p.num_m_tiles = B * p.tiles_x * p.tiles_y;
-    p.kchunks = (Cin + BK - 1) / BK;
+    p.kchunks = (Cin + E::kBK - 1) / E::kBK;
     p.num_kb = ntaps * p.kchunks;
     p.M = B * H * Wd; p.N = Cout; p.K = ntaps * Cin;
     p.nimg = B;
+    p.a_scale = a_scale; p.w_scale = w_scale;
     int rc = fill_epilogue(p, ep, Cout);
     if (rc) return rc;
     SUPIR_REQUIRE(ldc >= p.n_out, "%s: ldc %lld < output columns %d", who, ldc, p.n_out);
@@ -795,9 +801,9 @@ static int conv_geom_impl(const char* who, const void* x, long long ldx, const v
     CUtensorMap tmA;
     const uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)Win, (uint64_t)Hin, (uint64_t)B};
     const uint64_t str[3] = {(uint64_t)ldx, (uint64_t)ldx * Win, (uint64_t)ldx * Win * Hin};
-    const uint32_t box[4] = {BK, (uint32_t)(p.TW * g.stride), (uint32_t)(p.TH * g.stride), 1};
+    const uint32_t box[4] = {(uint32_t)E::kBK, (uint32_t)(p.TW * g.stride), (uint32_t)(p.TH * g.stride), 1};
     const uint32_t est[4] = {1, (uint32_t)g.stride, (uint32_t)g.stride, 1};
-    rc = make_tmap_16(&tmA, E::kTma, x, 4, dims, str, box, 128, est);
+    rc = make_tmap_16(&tmA, E::kOpTma, x, 4, dims, str, box, 128, est, E::kOpBytes);
     if (rc) return rc;
     return run_gemm<E>(tmA, Wp, p.K, p, reinterpret_cast<cudaStream_t>(stream));
 }
@@ -857,4 +863,22 @@ extern "C" int supir_conv3x3_bf16(const void* x, long long ldx, const void* Wp, 
 extern "C" int supir_conv3x3_f16(const void* x, long long ldx, const void* Wp, void* out, long long ldc, int B, int H,
                                  int Wd, int Cin, int Cout, const supir_epilogue* ep, void* stream) {
     return conv_geom_impl<F16>("supir_conv3x3_f16", x, ldx, Wp, out, ldc, B, H, Wd, Cin, Cout, conv3x3_geometry(H, Wd), ep, stream);
+}
+
+extern "C" int supir_conv3x3_fp8(const void* x, long long ldx, const float* x_scale, const void* Wp, const float* w_scale, void* out,
+                                 long long ldc, int B, int H, int Wd, int Cin, int Cout, const supir_epilogue* ep, void* stream) {
+    const char* who = "supir_conv3x3_fp8";
+    const auto al = [](const void* q, int b) { return (reinterpret_cast<uintptr_t>(q) & (b - 1)) == 0; };
+    SUPIR_REQUIRE(x && Wp && out && x_scale && w_scale, "%s: null pointer", who);
+    SUPIR_REQUIRE(B > 0 && H > 0 && Wd > 0 && Cin > 0 && Cout > 0, "%s: bad shape B=%d H=%d W=%d Cin=%d Cout=%d", who, B, H, Wd, Cin,
+                  Cout);
+    SUPIR_REQUIRE(Cin % 16 == 0 && ldx % 16 == 0 && ldx >= Cin,
+                  "%s: Cin and ldx must be multiples of 16 (16-byte TMA strides of e4m3), ldx >= Cin; got Cin=%d ldx=%lld", who, Cin, ldx);
+    SUPIR_REQUIRE(al(x, 16) && al(Wp, 16), "%s: x and Wp must be 16-byte aligned", who);
+    SUPIR_REQUIRE(al(x_scale, 4) && al(w_scale, 4), "%s: scales must be 4-byte aligned fp32", who);
+    SUPIR_REQUIRE(al(out, 2) && (!ep || !ep->residual || al(ep->residual, 2)), "%s: out / residual must be 2-byte aligned bf16", who);
+    SUPIR_REQUIRE(!ep || (!ep->out_f32 && !ep->ln_stats && !ep->ln_colsum && ep->act != 2),
+                  "%s: the FP8 conv epilogue writes bf16 and takes bias / rowvec / residual / SiLU only (no out_f32, ln_stats, GEGLU)",
+                  who);
+    return conv_geom_impl<E4m3>(who, x, ldx, Wp, out, ldc, B, H, Wd, Cin, Cout, conv3x3_geometry(H, Wd), ep, stream, x_scale, w_scale);
 }

@@ -210,6 +210,92 @@ __global__ void gn_apply_kernel(const typename E::T* __restrict__ x, long long l
 }
 
 // ---------------------------------------------------------------------------------------------
+// GroupNorm [+ SiLU] apply written as e4m3 for supir_conv3x3_fp8 (the ResBlocks' 3x3 convolutions in the FP8 convs mode): codes
+// q [B*HW, ldq] and one scale per image, scale[b] = amax / 448 over that image's fp32 apply values (e4m3_row_scale; no 16-bit
+// rounding in between). Two passes over x: gn_amax_kernel folds each block's max |value| into amax[b] (atomicMax on the bits
+// of a non-negative float: a max does not depend on the order, so the result is deterministic), then gn_apply_quant_kernel
+// computes the same fp32 values again (gn_value, the arithmetic of gn_apply_kernel) and writes the codes. Per-image scales
+// keep the images of a batch independent of each other. Same block layout as gn_apply_kernel.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float gn_value(float v, float sc, float sh, int silu) {
+    const float a = v * sc + sh;
+    return silu ? silu_f(a) : a;
+}
+
+__global__ void gn_amax_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int HW, int C, int G,
+                               const double* __restrict__ sums, double count, const float* __restrict__ gamma,
+                               const float* __restrict__ beta, float eps, int silu, int pixels_per_block,
+                               unsigned int* __restrict__ amax) {
+    __shared__ unsigned int block_max;
+    const int cv_count = C >> 3;
+    const int kp = blockDim.x / cv_count;
+    const int cv = threadIdx.x % cv_count;
+    const int pl = threadIdx.x / cv_count;            // >= kp: a thread of the last warp's padding, no pixels
+    const int b = blockIdx.y;
+    if (threadIdx.x == 0) block_max = 0u;
+    float sc[8], sh[8];
+    gn_scale_shift(b, cv * 8, C, G, sums, count, nullptr, nullptr, gamma, beta, eps, sc, sh);
+    const int p0 = blockIdx.x * pixels_per_block;
+    const int p1 = min(p0 + pixels_per_block, HW);
+    const __nv_bfloat16* xb = x + ((long long)b * HW) * ldx + cv * 8;
+    float m = 0.f;
+    for (int p = p0 + pl; pl < kp && p < p1; p += kp) {
+        const uint4 u = __ldg(reinterpret_cast<const uint4*>(xb + (long long)p * ldx));
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+            const float2 f = unpack_bf16x2(w[t]);
+            m = fmaxf(m, fmaxf(fabsf(gn_value(f.x, sc[2 * t], sh[2 * t], silu)), fabsf(gn_value(f.y, sc[2 * t + 1], sh[2 * t + 1], silu))));
+        }
+    }
+    m = warp_max(m);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) atomicMax(&block_max, __float_as_uint(m));
+    __syncthreads();
+    if (threadIdx.x == 0) atomicMax(amax + b, block_max);
+}
+
+__global__ void gn_apply_quant_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, uint8_t* __restrict__ q, long long ldq,
+                                      float* __restrict__ scale, const unsigned int* __restrict__ amax, int HW, int C, int G,
+                                      const double* __restrict__ sums, double count, const float* __restrict__ gamma,
+                                      const float* __restrict__ beta, float eps, int silu, int pixels_per_block) {
+    const int cv_count = C >> 3;
+    const int kp = blockDim.x / cv_count;
+    const int cv = threadIdx.x % cv_count;
+    const int pl = threadIdx.x / cv_count;
+    const int b = blockIdx.y;
+    float s, inv;
+    e4m3_row_scale(__uint_as_float(amax[b]), s, inv);
+    if (blockIdx.x == 0 && threadIdx.x == 0) scale[b] = s;
+    float sc[8], sh[8];
+    gn_scale_shift(b, cv * 8, C, G, sums, count, nullptr, nullptr, gamma, beta, eps, sc, sh);
+    const int p0 = blockIdx.x * pixels_per_block;
+    const int p1 = min(p0 + pixels_per_block, HW);
+    const __nv_bfloat16* xb = x + ((long long)b * HW) * ldx + cv * 8;
+    uint8_t* qb = q + ((long long)b * HW) * ldq + cv * 8;
+    auto one = [&](const uint4 u, long long p) {
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+        float v[8];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+            const float2 f = unpack_bf16x2(w[t]);
+            v[2 * t] = gn_value(f.x, sc[2 * t], sh[2 * t], silu) * inv;
+            v[2 * t + 1] = gn_value(f.y, sc[2 * t + 1], sh[2 * t + 1], silu) * inv;
+        }
+        __stcs(reinterpret_cast<uint2*>(qb + p * ldq), make_uint2(pack_e4m3x4(v[0], v[1], v[2], v[3]), pack_e4m3x4(v[4], v[5], v[6], v[7])));
+    };
+    int p = p0 + pl;
+    for (; p + 3 * kp < p1; p += 4 * kp) {      // four independent 16-byte loads in flight per thread
+        const uint4 u0 = __ldg(reinterpret_cast<const uint4*>(xb + (long long)p * ldx));
+        const uint4 u1 = __ldg(reinterpret_cast<const uint4*>(xb + (long long)(p + kp) * ldx));
+        const uint4 u2 = __ldg(reinterpret_cast<const uint4*>(xb + (long long)(p + 2 * kp) * ldx));
+        const uint4 u3 = __ldg(reinterpret_cast<const uint4*>(xb + (long long)(p + 3 * kp) * ldx));
+        one(u0, p); one(u1, p + kp); one(u2, p + 2 * kp); one(u3, p + 3 * kp);
+    }
+    for (; p < p1; p += kp) one(__ldg(reinterpret_cast<const uint4*>(xb + (long long)p * ldx)), p);
+}
+
+// ---------------------------------------------------------------------------------------------
 // ZeroSFT tail (SUPIR_v0.py:110-113): out = lerp(h_raw, GN(h) * (gamma + 1) + beta, control_scale)
 //   h      : [B, HW, C]  (= cat(h_ori, skip + zero_conv(c)))        gb : [B, HW, 2C] = (gamma | beta) conv outputs
 //   h_raw first C1 channels equal h's; the remaining C - C1 come from `skip_raw` [B, HW, C - C1]
@@ -562,6 +648,38 @@ extern "C" int supir_groupnorm_apply_f16(const void* x, long long ldx, void* y, 
                                          const float* gamma, const float* beta, float eps, int silu, void* stream) {
     return groupnorm_apply_impl<F16>("supir_groupnorm_apply_f16", x, ldx, y, ldy, B, HW, C, groups, sums, mean, var, gamma, beta,
                                      eps, silu, stream);
+}
+
+extern "C" int supir_groupnorm_apply_quant(const void* x, long long ldx, void* q, long long ldq, float* scale, unsigned int* amax_ws,
+                                           int B, int HW, int C, int groups, const double* sums, const float* gamma,
+                                           const float* beta, float eps, int silu, void* stream) {
+    const char* who = "supir_groupnorm_apply_quant";
+    const auto al = [](const void* p, int b) { return (reinterpret_cast<uintptr_t>(p) & (b - 1)) == 0; };
+    SUPIR_REQUIRE(x && q && scale && amax_ws && sums, "%s: null pointer", who);
+    SUPIR_REQUIRE(B > 0 && HW > 0, "%s: bad shape B=%d HW=%d", who, B, HW);
+    SUPIR_REQUIRE(groups > 0 && C % 16 == 0 && C % groups == 0 && C <= 8192 && ldx % 8 == 0 && ldx >= C && ldq % 16 == 0 && ldq >= C,
+                  "%s: unsupported C=%d groups=%d ldx=%lld ldq=%lld (C, ldq multiples of 16, ldx of 8)", who, C, groups, ldx, ldq);
+    SUPIR_REQUIRE(al(x, 16) && al(q, 16) && al(scale, 4) && al(amax_ws, 4), "%s: misaligned pointer (x, q: 16 bytes; scale, amax_ws: 4)",
+                  who);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const int cvc = C >> 3;
+    int kp = 512 / cvc;
+    if (kp < 1) kp = 1;
+    const int threads = kp * cvc;
+    int ppb = kp * 32;
+    if (ppb > HW) ppb = (HW + kp - 1) / kp * kp;
+    const int bx = (HW + ppb - 1) / ppb;
+    const double count = (double)HW * (C / groups);
+    const __nv_bfloat16* xp = reinterpret_cast<const __nv_bfloat16*>(x);
+    // the accumulator is reset on the stream (a memset node inside a captured graph), never by the host
+    SUPIR_CHECK_CUDA(cudaMemsetAsync(amax_ws, 0, sizeof(unsigned int) * B, st));
+    gn_amax_kernel<<<dim3(bx, B), (threads + 31) / 32 * 32, 0, st>>>(xp, ldx, HW, C, groups, sums, count, gamma, beta, eps, silu, ppb,
+                                                                      amax_ws);
+    gn_apply_quant_kernel<<<dim3(bx, B), threads, 0, st>>>(xp, ldx, reinterpret_cast<uint8_t*>(q), ldq, scale, amax_ws, HW, C, groups,
+                                                           sums, count, gamma, beta, eps, silu, ppb);
+    count_launch(2);
+    SUPIR_CHECK_CUDA(cudaGetLastError());
+    return SUPIR_OK;
 }
 
 template <class E>

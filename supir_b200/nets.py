@@ -7,7 +7,8 @@ path: `pack(dtype)` converts the weights once into the kernel layouts (bf16 or f
 gamma|beta matrices, fp32 biases) and `run()` issues hand-written sm_90a kernels through the C ABI (supir_b200/ops.py) on
 channels-last activations of that dtype (torch.autocast(bfloat16) or autocast(float16) numerics). `pack(float8_e4m3fn)` is
 the bf16 pack except for the Linear layers inside every BasicTransformerBlock, which hold e4m3 weights with per-row scales and
-run on FP8 tensor cores (see `linear`). Options the SUPIR configs never use raise NotImplementedError.
+run on FP8 tensor cores (see `linear`); `pack(float8_e4m3fn, fp8_convs=True)` also runs the two 3x3 convolutions of every
+ResBlock on them (see `ResBlock.run`). Options the SUPIR configs never use raise NotImplementedError.
 """
 import os
 
@@ -121,6 +122,16 @@ def group_norm(ctx, x: Act, norm: nn.GroupNorm, silu, out=None):
     return Act(o, x.B, x.H, x.W)
 
 
+def group_norm_silu_quant(ctx, x: Act, norm: nn.GroupNorm):
+    """SiLU(GroupNorm(x)) as conv3x3_fp8's operand: (e4m3 codes [rows, C], fp32 scale [B], one per image)."""
+    sums = ctx.pool.get((ops.groupnorm_ws_size(x.B, x.HW, x.C),), torch.float64)
+    ops.groupnorm_stats(x.t, x.B, x.HW, sums)
+    q, sc, amax = ctx.new(x.rows, x.C, ops.FP8), ctx.pool.get((x.B,), torch.float32), ctx.pool.get((x.B,), torch.int32)
+    ops.groupnorm_apply_quant(x.t, x.B, x.HW, q, sc, amax, norm._w, norm._b, norm.eps, True, sums)
+    ctx.pool.put(sums, amax)
+    return q, sc
+
+
 def pack_norm(n):
     n._w, n._b = _f32(n.weight), _f32(n.bias)
 
@@ -167,22 +178,37 @@ class ResBlock(nn.Module):
         self.skip_connection = nn.Identity() if self.out_channels == channels else nn.Conv2d(channels, self.out_channels, 1)
         self.emb_offset = None
 
+    fp8_convs = False   # set by the network's pack(float8_e4m3fn, fp8_convs=True): e4m3 in_layers.2 / out_layers.3
+
     def pack(self, dtype=BF16):
         pack_norm(self.in_layers[0]), pack_norm(self.out_layers[0])
-        self._w1, self._b1 = pack_conv3x3(self.in_layers[2].weight, dtype), _bias_values(self.in_layers[2].bias, dtype)
-        self._w2, self._b2 = pack_conv3x3(self.out_layers[3].weight, dtype), _bias_values(self.out_layers[3].bias, dtype)
+        # FP8: (e4m3 codes, one scale per output channel) of the bf16 packed matrix [Cout, 9*Cin]; the bf16 copy is not kept
+        conv = (lambda w: ops.quantize_weight(pack_conv3x3(w, dtype))) if self.fp8_convs else (lambda w: pack_conv3x3(w, dtype))
+        self._w1, self._b1 = conv(self.in_layers[2].weight), _bias_values(self.in_layers[2].bias, dtype)
+        self._w2, self._b2 = conv(self.out_layers[3].weight), _bias_values(self.out_layers[3].bias, dtype)
         if isinstance(self.skip_connection, nn.Conv2d):
             self._ws = _bf(self.skip_connection.weight.reshape(self.out_channels, self.channels), dtype)
             self._bs = _bias_values(self.skip_connection.bias, dtype)
 
+    def _norm_silu(self, ctx, x: Act, norm):
+        """The input of a 3x3 convolution: an Act, or packed FP8 the (codes, per-image scales) pair of conv3x3_fp8."""
+        return group_norm_silu_quant(ctx, x, norm) if self.fp8_convs else group_norm(ctx, x, norm, silu=True)
+
+    def _conv(self, ctx, n, x: Act, w, out, **kw):
+        if self.fp8_convs:
+            ops.conv3x3_fp8(*n, x.B, x.H, x.W, *w, out, **kw)
+            ctx.free(*n)
+        else:
+            ops.conv3x3(n.t, x.B, x.H, x.W, w, out, **kw)
+            ctx.free(n)
+
     def run(self, ctx, x: Act):
-        n1 = group_norm(ctx, x, self.in_layers[0], silu=True)
+        n1 = self._norm_silu(ctx, x, self.in_layers[0])
         emb = ctx.emb_all[:, self.emb_offset:self.emb_offset + self.out_channels]
         h = ctx.new(x.rows, self.out_channels)
-        ops.conv3x3(n1.t, x.B, x.H, x.W, self._w1, h, bias=self._b1, rowvec=emb)
-        ctx.free(n1)
+        self._conv(ctx, n1, x, self._w1, h, bias=self._b1, rowvec=emb)
         hA = Act(h, x.B, x.H, x.W)
-        n2 = group_norm(ctx, hA, self.out_layers[0], silu=True)
+        n2 = self._norm_silu(ctx, hA, self.out_layers[0])
         ctx.free(hA)
         if isinstance(self.skip_connection, nn.Conv2d):
             skip = ctx.new(x.rows, self.out_channels)
@@ -190,8 +216,7 @@ class ResBlock(nn.Module):
         else:
             skip = x.t
         out = ctx.new(x.rows, self.out_channels)
-        ops.conv3x3(n2.t, x.B, x.H, x.W, self._w2, out, bias=self._b2, residual=skip)
-        ctx.free(n2)
+        self._conv(ctx, n2, x, self._w2, out, bias=self._b2, residual=skip)
         if skip is not x.t:
             ctx.free(skip)
         return Act(out, x.B, x.H, x.W)
@@ -604,20 +629,25 @@ class _UNetBase(nn.Module):
         return chans, ch, ds, ted, transformer_depth, st
 
     # ---- packing -----------------------------------------------------------------------------------------------------
-    def pack(self, dtype=BF16):
+    def pack(self, dtype=BF16, fp8_convs=False):
         """Convert parameters into kernel layouts (call again after load_state_dict / .to()). `dtype` is the compute dtype:
         torch.bfloat16, or torch.float16 for the fp16 mode (every 16-bit weight, bias value and activation in fp16), or
         torch.float8_e4m3fn for the FP8 mode: bf16 everywhere except the Linear layers of every BasicTransformerBlock (QKV,
         to_out, the cross-attention's to_q, GEGLU, ff.net.2), which hold e4m3 weights with one fp32 scale per output channel
-        and take e4m3 activations with one scale per row."""
+        and take e4m3 activations with one scale per row. `fp8_convs` (FP8 mode only) also runs the two 3x3 convolutions of
+        every ResBlock (in_layers.2, out_layers.3) on e4m3 weights with one scale per output channel and e4m3 activations with
+        one scale per image (the GroupNorm + SiLU in front of them writes them)."""
         if dtype not in (BF16, ops.F16, ops.FP8):
             raise ValueError(f"compute dtype {dtype} is not supported (bfloat16, float16 or float8_e4m3fn)")
+        if fp8_convs and dtype != ops.FP8:
+            raise ValueError(f"fp8_convs needs the float8_e4m3fn compute dtype (got {dtype})")
         fp8 = dtype == ops.FP8
         dtype = BF16 if fp8 else dtype
         res, xattn = [], []
         for m in self.modules():
             if isinstance(m, ResBlock):
                 res.append(m)
+                m.fp8_convs = bool(fp8_convs)
             if isinstance(m, BasicTransformerBlock):
                 xattn.append(m.attn2)
                 m.fp8 = fp8
@@ -645,6 +675,7 @@ class _UNetBase(nn.Module):
         self._packed_device = self._emb_w.device
         self._packed_dtype = dtype
         self._fp8_linears = fp8
+        self._fp8_convs = bool(fp8_convs)
         return self
 
     def project_context(self, context_16, out):
@@ -753,8 +784,8 @@ class LightGLVUNet(_UNetBase):
         for i in [6, 3]:
             self.project_modules.insert(i, ZeroCrossAttn(cond_output_channels[i], concat_channels[i]))
 
-    def pack(self, dtype=BF16):
-        super().pack(dtype)
+    def pack(self, dtype=BF16, fp8_convs=False):
+        super().pack(dtype, fp8_convs)
         dtype = self._packed_dtype
         pack_norm(self.out[0])
         w = self.out[2].weight.detach()

@@ -8,7 +8,9 @@ The ops the diffusion networks use also take fp16 operands (their fp16 compute m
 `_f16` twin from the dtype of its 16-bit operands, and refuses operands that mix the two before anything is launched.
 
 FP8 linear layers (the networks' float8_e4m3fn mode): gemm_fp8 multiplies e4m3 operands with one fp32 scale per row of each
-(quantize_weight at pack time; quantize_rows / layernorm_quant for the activations) into a bf16 result.
+(quantize_weight at pack time; quantize_rows / layernorm_quant for the activations) into a bf16 result. FP8 convolutions (the
+fp8_convs option of that mode): conv3x3_fp8 takes e4m3 activations with one scale per image (groupnorm_apply_quant) and e4m3
+weights with one scale per output channel (quantize_weight of the packed [Cout, 9*Cin] matrix).
 """
 import ctypes
 
@@ -210,6 +212,30 @@ def conv3x3(x, B, H, W, wp, out, bias=None, rowvec=None, residual=None, act=0):
     return out
 
 
+def conv3x3_fp8(x_q, x_scale, B, H, W, w_q, w_scale, out, bias=None, rowvec=None, residual=None, act=0):
+    """3x3/s1/p1 conv on e4m3 operands (supir_conv3x3_fp8): x_q [B*H*W, Cin] NHWC codes with one fp32 scale per image,
+    x_scale [B]; w_q [Cout, 9*Cin] codes packed like conv3x3's weight with one fp32 scale per output channel, w_scale [Cout];
+    out[p, n] = epilogue(x_scale[image of p] * w_scale[n] * acc) with conv3x3's bf16 epilogue (bias, rowvec, SiLU, residual)."""
+    if x_q.dtype != FP8 or w_q.dtype != FP8:
+        raise TypeError(f"conv3x3_fp8: operands must both be float8_e4m3fn (got {x_q.dtype}, {w_q.dtype})")
+    if out.dtype != BF16 or (residual is not None and residual.dtype != BF16):
+        raise TypeError("conv3x3_fp8: out and residual are bfloat16")
+    if x_scale.dtype != torch.float32 or w_scale.dtype != torch.float32:
+        raise TypeError("conv3x3_fp8: scales are float32")
+    if act not in (0, 1):
+        raise ValueError("conv3x3_fp8: act is 0 (none) or 1 (SiLU)")
+    _need_cuda(x_q, x_scale, w_q, w_scale, out)
+    _mat(x_q, FP8), _mat(w_q, FP8)
+    Cin, Cout = x_q.shape[1], w_q.shape[0]
+    assert x_q.shape[0] == B * H * W and w_q.shape[1] == 9 * Cin and w_q.is_contiguous() and out.shape == (B * H * W, Cout), \
+        (x_q.shape, w_q.shape, out.shape, B, H, W)
+    assert x_scale.shape == (B,) and w_scale.shape == (Cout,) and x_scale.is_contiguous() and w_scale.is_contiguous()
+    ep = _epilogue(bias, rowvec, 0, residual, act, False)
+    call("supir_conv3x3_fp8", _ptr(x_q), x_q.stride(0), _ptr(x_scale), _ptr(w_q), _ptr(w_scale), _ptr(out), out.stride(0), B, H, W,
+         Cin, Cout, ctypes.byref(ep), _stream())
+    return out
+
+
 def conv_geom(x, B, Hin, Win, wp, out, geom, bias=None, act=0):
     """General small-kernel convolution (see supir_conv_geometry): x [B*Hin*Win, Cin], wp [Cout, kh*kw*Cin], out [B*out_H*out_W, Cout]."""
     name = _entry("supir_conv_geom_bf16", x, wp, out)
@@ -327,6 +353,24 @@ def groupnorm_apply(x, B, HW, out, gamma, beta, eps, silu, sums=None, mean=None,
     call(name, _ptr(x), x.stride(0), _ptr(out), out.stride(0), B, HW, x.shape[1], groups, _ptr(sums),
          _ptr(mean), _ptr(var), _ptr(gamma), _ptr(beta), float(eps), int(silu), _stream())
     return out
+
+
+def groupnorm_apply_quant(x, B, HW, q, scale, amax_ws, gamma, beta, eps, silu, sums, groups=32):
+    """GroupNorm [+ SiLU] of bf16 x [B*HW, C] written as conv3x3_fp8's operand: q (e4m3, x's shape) and scale (fp32 [B]), one
+    scale per image from the amax of the fp32 apply values (no bf16 rounding in between), per e4m3_row_scales of the image's
+    values. `sums` from groupnorm_stats; amax_ws: int32 [B] scratch (reset by the call on the stream)."""
+    if x.dtype != BF16 or q.dtype != FP8 or scale.dtype != torch.float32 or amax_ws.dtype != torch.int32:
+        raise TypeError(f"groupnorm_apply_quant: bfloat16 -> float8_e4m3fn + float32, int32 scratch (got {x.dtype}, {q.dtype}, "
+                        f"{scale.dtype}, {amax_ws.dtype})")
+    if sums is None or sums.dtype != torch.float64:
+        raise TypeError("groupnorm_apply_quant: sums are the float64 output of groupnorm_stats")
+    _need_cuda(x, q, scale, amax_ws, sums)
+    _mat(x), _mat(q, FP8)
+    assert q.shape == x.shape and x.shape[0] == B * HW and scale.shape == (B,) and amax_ws.shape == (B,), (x.shape, q.shape, B, HW)
+    assert scale.is_contiguous() and amax_ws.is_contiguous()
+    call("supir_groupnorm_apply_quant", _ptr(x), x.stride(0), _ptr(q), q.stride(0), _ptr(scale), _ptr(amax_ws), B, HW, x.shape[1],
+         groups, _ptr(sums), _ptr(gamma), _ptr(beta), float(eps), int(silu), _stream())
+    return q, scale
 
 
 def zerosft_apply(h, skip_raw, C1, gamma_beta, out, B, HW, sums, gn_w, gn_b, eps, control_scale, groups=32):

@@ -1,12 +1,14 @@
-"""python tools/bench_fp8.py [--out DIR] : bf16 against the FP8 linears mode (ControlWrapper.dtype = torch.float8_e4m3fn) on
-the bench's networks (SUPIR-v0 + SDXL-base shapes, random weights), in one process:
+"""python tools/bench_fp8.py [--out DIR] : bf16 against the FP8 linears mode (ControlWrapper.dtype = torch.float8_e4m3fn) and the
+FP8 linears + convs mode (also ControlWrapper.fp8_convs = True) on the bench's networks (SUPIR-v0 + SDXL-base shapes, random
+weights), in one process:
 
-  1. one denoiser call of the bench plan (34 rows = 17 windows x CFG pair of 128^2 latent), bf16 and FP8 alternated 3x each,
-     CUDA events around 5 graph replays per window, with the card, its power limit and the median SM clock of each window;
-  2. the per-launch shape table of one eager FP8 call (the SUPIR_BENCH_DUMP_SHAPES form of bench.py), GEMM-class launches and
-     the quantization passes (layernorm_quant, quantize_rows) each timed with a CUDA-event pair;
-  3. the cfg3 EDM step (49 windows, tile batch 17) in both modes, alternated, without the VAE (a random latent);
-  4. the resident bytes of the packed networks in both modes.
+  1. one denoiser call of the bench plan (34 rows = 17 windows x CFG pair of 128^2 latent), bf16 / FP8 / FP8 + convs alternated
+     3x each, CUDA events around 5 graph replays per window, with the card, its power limit and the median SM clock of each window;
+  2. the per-launch shape table of one eager call in each mode (the SUPIR_BENCH_DUMP_SHAPES form of bench.py), GEMM-class
+     launches (gemm, gemm_fp8, conv3x3, conv3x3_fp8), the quantization passes (layernorm_quant, quantize_rows) and the GroupNorm
+     applies (groupnorm_apply, groupnorm_apply_quant) each timed with a CUDA-event pair;
+  3. the cfg3 EDM step (49 windows, tile batch 17) in the three modes, alternated, without the VAE (a random latent);
+  4. the resident bytes of the packed networks in each mode.
 
 Prints one JSON line and writes it (and the shape table) under --out. Reuses bench.engine_config / ClockSampler unchanged."""
 import argparse
@@ -24,7 +26,7 @@ sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 
 FP8, BF = torch.float8_e4m3fn, torch.bfloat16
-MODES = {"bf16": BF, "fp8": FP8}
+MODES = {"bf16": (BF, False), "fp8": (FP8, False), "fp8_convs": (FP8, True)}     # (ControlWrapper.dtype, .fp8_convs)
 
 
 def card():
@@ -48,7 +50,7 @@ def packed_bytes(net):
 
 
 def set_mode(net, mode):
-    net.dtype = MODES[mode]
+    net.dtype, net.fp8_convs = MODES[mode]
     net.pack()
     torch.cuda.empty_cache()
 
@@ -70,7 +72,8 @@ def time_call(net, args, reps):
 
 
 def shape_table(net):
-    """One eager run of the captured plan with a CUDA-event pair around every GEMM-class and quantization launch."""
+    """One eager run of the captured plan with a CUDA-event pair around every GEMM-class, quantization and GroupNorm-apply launch.
+    Memory-bound rows report GB/s from the bytes per element they move (`gbs`)."""
     from supir_b200 import ops
     rec, orig = [], {}
 
@@ -83,7 +86,8 @@ def shape_table(net):
             e0.record()
             r = f(*a, **kw)
             e1.record()
-            rec.append((e0, e1) + flop(*a, **kw))
+            fl = flop(*a, **kw)
+            rec.append((e0, e1, fl[0], fl[1], fl[2] if len(fl) > 2 else 0))
             return r
         setattr(ops, name, g)
 
@@ -91,8 +95,13 @@ def shape_table(net):
     wrap("gemm_fp8", lambda aq, sa, wq, sw, out, **kw: (2.0 * aq.shape[0] * wq.shape[0] * aq.shape[1],
                                                        ("gemm_fp8", aq.shape[0], wq.shape[0], aq.shape[1], kw.get("act", 0))))
     wrap("conv3x3", lambda x, B, H, W, wp, out, **kw: (2.0 * x.shape[0] * wp.shape[0] * wp.shape[1], ("conv3x3", x.shape[0], wp.shape[0], wp.shape[1], kw.get("act", 0))))
-    wrap("quantize_rows", lambda x, q, s: (0.0, ("quantize_rows", x.shape[0], 0, x.shape[1], 0)))
-    wrap("layernorm_quant", lambda x, g, b, q, s, eps=1e-5: (0.0, ("layernorm_quant", x.shape[0], 0, x.shape[1], 0)))
+    wrap("conv3x3_fp8", lambda xq, xs, B, H, W, wq, ws, out, **kw: (2.0 * xq.shape[0] * wq.shape[0] * wq.shape[1],
+                                                                  ("conv3x3_fp8", xq.shape[0], wq.shape[0], wq.shape[1], kw.get("act", 0))))
+    # bytes per element: bf16 read + e4m3 write (3), bf16 read + bf16 write (4), bf16 read twice + e4m3 write (5)
+    wrap("quantize_rows", lambda x, q, s: (0.0, ("quantize_rows", x.shape[0], 0, x.shape[1], 0), 3))
+    wrap("layernorm_quant", lambda x, g, b, q, s, eps=1e-5: (0.0, ("layernorm_quant", x.shape[0], 0, x.shape[1], 0), 3))
+    wrap("groupnorm_apply", lambda x, B, HW, out, *a, **kw: (0.0, ("groupnorm_apply", x.shape[0], 0, x.shape[1], 0), 4))
+    wrap("groupnorm_apply_quant", lambda x, B, HW, *a, **kw: (0.0, ("groupnorm_apply_quant", x.shape[0], 0, x.shape[1], 0), 5))
     plan = next(iter(net._plans.values()))
     try:
         plan._run()
@@ -101,14 +110,14 @@ def shape_table(net):
         for k, f in orig.items():
             setattr(ops, k, f)
     agg = {}
-    for e0, e1, fl, key in rec:
-        a = agg.setdefault(key, [0, 0.0, 0.0])
+    for e0, e1, fl, key, bpe in rec:
+        a = agg.setdefault(key, [0, 0.0, 0.0, bpe])
         a[0] += 1
         a[1] += e0.elapsed_time(e1)
         a[2] += fl
     rows = sorted(({"op": k[0], "M": k[1], "N": k[2], "K": k[3], "act": k[4], "count": v[0], "ms": round(v[1], 3),
                     "tflops": round(v[2] / (v[1] * 1e-3) / 1e12, 1) if v[2] else None,
-                    "gbs": round(k[1] * k[3] * 3 / (v[1] / v[0] * 1e-3) / 1e9, 1) if not v[2] else None}
+                    "gbs": round(k[1] * k[3] * v[3] / (v[1] / v[0] * 1e-3) / 1e9, 1) if not v[2] else None}
                    for k, v in agg.items()), key=lambda r: -r["ms"])
     return {"total_ms": sum(r["ms"] for r in rows), "rows": rows}
 
@@ -131,18 +140,16 @@ def main():
             "control": torch.randn(B, 4, 128, 128, device="cuda")}
     t = torch.full((B,), 500.0, device="cuda")
     call_args = (x, t, cond)
-    calls = {"bf16": [], "fp8": []}
+    calls = {mode: [] for mode in MODES}
     res["resident_bytes"] = {}
     for rep in range(3):
-        for mode in ("bf16", "fp8"):
+        for mode in MODES:
             set_mode(net, mode)
             res["resident_bytes"][mode] = packed_bytes(net)
             ms, clk = time_call(net, call_args, args.reps)
             calls[mode].append({"ms": ms, "sm_mhz": clk.get("sm_mhz"), "reasons": clk.get("reasons")})
-            if mode == "fp8" and rep == 2:
-                res["fp8_shape_table"] = shape_table(net)
-            if mode == "bf16" and rep == 2:
-                res["bf16_shape_table"] = shape_table(net)
+            if rep == 2:
+                res[f"{mode}_shape_table"] = shape_table(net)
     res["call_34rows_128"] = {k: {"median_ms": float(np.median([c["ms"] for c in v])), "windows": v} for k, v in calls.items()}
     # ---- 3. the cfg3 EDM step (no VAE: a random latent) ----
     from supir_b200 import sampling
@@ -150,9 +157,9 @@ def main():
     c = {"crossattn": torch.randn(1, 77, 2048, device="cuda"), "vector": torch.randn(1, 2816, device="cuda")}
     uc = {"crossattn": torch.randn(1, 77, 2048, device="cuda"), "vector": torch.randn(1, 2816, device="cuda")}
     z = 0.5 * torch.randn(1, 4, latent, latent, device="cuda")
-    steps = {"bf16": [], "fp8": []}
+    steps = {mode: [] for mode in MODES}
     for rep in range(3):
-        for mode in ("bf16", "fp8"):
+        for mode in MODES:
             set_mode(net, mode)
             smp = m.make_sampler(w["steps"], -1.0, 5, 1.01, 4.0, True, 1.0)
             run = smp.begin(sampling.FusedDenoiser(m.denoiser, net), torch.randn_like(z), dict(c, control=z), dict(uc, control=z),
@@ -182,6 +189,13 @@ def main():
         json.dump(res, f, indent=1)
     short = {k: v for k, v in res.items() if not k.endswith("shape_table")}
     short["fp8_shape_table_top"] = res["fp8_shape_table"]["rows"][:12]
+    short["fp8_convs_shape_table_top"] = res["fp8_convs_shape_table"]["rows"][:12]
+    # the per-launch rows the convs option changes: 3x3 convolutions and GroupNorm applies, before (fp8) and after (fp8_convs)
+    conv_ops = ("conv3x3", "conv3x3_fp8", "groupnorm_apply", "groupnorm_apply_quant")
+    for mode in ("fp8", "fp8_convs"):
+        t = res[f"{mode}_shape_table"]["rows"]
+        short[f"{mode}_conv_rows"] = [r for r in t if r["op"] in conv_ops]
+        short[f"{mode}_ms_by_op"] = {op: round(sum(r["ms"] for r in t if r["op"] == op), 3) for op in sorted({r["op"] for r in t})}
     print(json.dumps(short))
 
 
