@@ -220,6 +220,7 @@ int supir_softmax_rows(const float* S, long long lds, void* P, long long ldp, lo
 /* K6: attention, head_dim 64 (attention.cu)                                                                          */
 /* ------------------------------------------------------------------------------------------------------------------ */
 /* out[b, i, h*64:(h+1)*64] = softmax(q_h k_h^T * scale) v_h ; q [B*Lq, ldq], k/v [B*Lk, ldk/ldv], head h at column h*64.
+ * Every leading dimension is a multiple of 8 and >= H*64; out is 4-byte aligned (outputs are stored in pairs).
  * Replaces F.scaled_dot_product_attention / xformers in CrossAttention (attention.py:273-277, 357-359) and
  * ZeroCrossAttn (SUPIR_v0.py:146). */
 int supir_attention_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
@@ -229,16 +230,26 @@ int supir_attention_f16(const void* q, long long ldq, const void* k, long long l
                         void* out, long long ldo, int B, int H, int Lq, int Lk, int head_dim, float scale, void* stream);
 /* Single-head attention with a wide head over L tokens per batch element (the SDXL VAE mid-block AttnBlock, head_dim 512:
  * model.py:158-206, 209-262; tilevae.py:292-336; 128 / 256 for reduced-width VAE configurations):
- * out[b, i, 0:head_dim] = softmax(q k^T * scale) v. q/k/v/out: [B*L, ld] bf16, ld >= head_dim. Flash-style (no score matrix
- * in HBM); at head_dim 512 the two halves of the value columns run as separate CTAs. */
+ * out[b, i, 0:head_dim] = softmax(q k^T * scale) v. q/k/v/out: [B*L, ld] bf16, ld a multiple of 8 and >= head_dim; out
+ * 4-byte aligned. Flash-style (no score matrix in HBM); at head_dim 512 the two halves of the value columns run as separate
+ * CTAs. */
 int supir_attention_1head_bf16(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                                void* out, long long ldo, int B, int L, int head_dim, float scale, void* stream);
-/* tuning knob: how many of every 4 element pairs of the softmax take 2^x from the FMA-pipe polynomial instead of MUFU.EX2
- * (0..4; default 0 = all on MUFU, or the environment variable SUPIR_B200_ATTN_EMU; negative restores the default). */
+/* Tuning knobs of the attention softmax (values above 4 clamp to 4; negative restores the default, which is 0 or the
+ * environment variable named below).
+ * supir_set_attention_exp_emulation: how many of every 4 element pairs take 2^x from the FMA-pipe polynomial instead of
+ * MUFU.EX2 (environment SUPIR_B200_ATTN_EMU). The online-softmax rescale factor always comes from MUFU.EX2.
+ * supir_set_attention_alu_pack: how many of every 4 probability pairs are rounded / packed to bf16 with integer instructions
+ * (round half up) on the ALU pipe instead of cvt.rn.bf16x2.f32, which shares the XU pipe with the exponentials (environment
+ * SUPIR_B200_ATTN_ALU_PACK).
+ * Each kernel compiles only some variants; the value set maps onto them as follows:
+ *   kernel                   | emulation 0, 1 | emulation 2 | emulation 3 | emulation 4 | ALU packing
+ *   head_dim 64, bf16        | none           | 2 of 4      | 2 of 4      | 2 of 4      | 0, 1 -> 2, 3, 4; ignored at emulation >= 2
+ *   head_dim 64, fp16        | none           | 2 of 4      | 2 of 4      | 2 of 4      | ignored
+ *   1-head, head_dim 512     | none           | 2 of 4      | none        | 4 of 4      | ignored
+ *   1-head, head_dim 128/256 | none           | none        | none        | none        | ignored
+ * ("none": every pair on MUFU; ALU packing 1 runs as 2.) tests/test_gpu_attention_fp64.py pins these classes. */
 int supir_set_attention_exp_emulation(int pairs_of_4);
-/* tuning knob: how many of every 4 probability pairs are rounded / packed to bf16 with integer instructions on the ALU pipe
- * instead of cvt.rn.bf16x2.f32, which shares the XU pipe with the exponentials (0..4; environment SUPIR_B200_ATTN_ALU_PACK;
- * negative restores the default). bf16 only: it has no effect on supir_attention_f16. */
 int supir_set_attention_alu_pack(int pairs_of_4);
 
 /* ------------------------------------------------------------------------------------------------------------------ */

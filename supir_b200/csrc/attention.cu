@@ -340,6 +340,10 @@ static int attention_h64_setup(const char* who, CUtensorMapDataType dt, CUtensor
     SUPIR_REQUIRE(B > 0 && H > 0 && Lq > 0 && Lk > 0, "%s: bad shape", who);
     SUPIR_REQUIRE(scale > 0.f, "%s: scale must be positive", who);
     SUPIR_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0, "%s: leading dims must be multiples of 8", who);
+    const long long cols = (long long)H * 64;
+    SUPIR_REQUIRE(ldq >= cols && ldk >= cols && ldv >= cols && ldo >= cols, "%s: leading dims must be >= H * 64 = %lld", who, cols);
+    // the final store writes two outputs as one 32-bit word
+    SUPIR_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0, "%s: out must be 4-byte aligned", who);
     int rc = make_attention_maps(dt, tmQ, tmK, tmV, q, ldq, k, ldk, v, ldv, (uint64_t)H * 64, (uint64_t)B * Lq, (uint64_t)B * Lk, 128);
     if (rc) return rc;
     *p = AttnParams{};
@@ -392,6 +396,7 @@ extern "C" int supir_attention_1head_bf16(const void* q, long long ldq, const vo
     SUPIR_REQUIRE(head_dim == 512 || head_dim == 256 || head_dim == 128, "supir_attention_1head_bf16: head_dim %d not in {128, 256, 512}", head_dim);
     SUPIR_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && ldq >= head_dim && ldk >= head_dim && ldv >= head_dim && ldo >= head_dim,
                   "supir_attention_1head_bf16: leading dims must be multiples of 8 and >= head_dim");
+    SUPIR_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0, "supir_attention_1head_bf16: out must be 4-byte aligned");
     CUtensorMap tmQ, tmK, tmV;
     int rc = make_attention_maps(Bf16::kTma, &tmQ, &tmK, &tmV, q, ldq, k, ldk, v, ldv, (uint64_t)head_dim, (uint64_t)B * L, (uint64_t)B * L, 64);
     if (rc) return rc;

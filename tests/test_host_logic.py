@@ -57,6 +57,31 @@ def test_text_conditioner_entry_points_reject_bad_arguments_before_any_launch():
         ops.attention_small(*(torch.zeros(77, 64, dtype=torch.bfloat16),) * 4, 1, 1, 77)      # CPU tensors: no fallback
 
 
+def test_attention_entry_points_reject_bad_arguments_before_any_launch():
+    """Argument validation of the attention.cu entry points: the final store writes two 16-bit outputs as one 32-bit word, so
+    `out` must be 4-byte aligned, and at head_dim 64 every leading dimension must cover the H * 64 columns (a shorter ldo
+    would let the last row write past the buffer). Both are rejected before any tensor map is encoded or anything launched."""
+    import ctypes
+    from supir_b200 import _native
+    lib = _native.load()
+    p = ctypes.c_void_p(64)            # a non-null, aligned dummy pointer; never dereferenced on these paths
+    odd = ctypes.c_void_p(66)          # 2-byte aligned: a bf16 view that starts at an odd column
+    h64 = lambda out, ldq, ldk, ldv, ldo: (p, ldq, p, ldk, p, ldv, out, ldo, 2, 5, 77, 77, 64, 0.125, None)  # noqa: E731
+    cases = []
+    for name in ("supir_attention_bf16", "supir_attention_f16"):
+        cases += [(name, h64(odd, 320, 320, 320, 320), "4-byte aligned"),
+                  (name, h64(p, 256, 320, 320, 320), ">= H * 64"),
+                  (name, h64(p, 320, 256, 320, 320), ">= H * 64"),
+                  (name, h64(p, 320, 320, 256, 320), ">= H * 64"),
+                  (name, h64(p, 320, 320, 320, 312), ">= H * 64")]
+    cases.append(("supir_attention_1head_bf16", (p, 512, p, 512, p, 512, odd, 512, 1, 100, 512, 0.04, None), "4-byte aligned"))
+    for name, args, needle in cases:
+        assert getattr(lib, name)(*args) < 0, name
+        assert needle in lib.supir_last_error().decode(), (name, lib.supir_last_error())
+        with pytest.raises(_native.SupirNativeError):
+            _native.call(name, *args)
+
+
 def test_no_cpu_fallback():
     from supir_b200 import _native, ops
     with pytest.raises(_native.SupirNativeError):
