@@ -252,6 +252,30 @@ int supir_attention_1head_bf16(const void* q, long long ldq, const void* k, long
 int supir_set_attention_exp_emulation(int pairs_of_4);
 int supir_set_attention_alu_pack(int pairs_of_4);
 
+/* FP8 attention, head_dim 64 (attention_fp8.cu; the fp8_attention option of the FP8 mode). Quantization, with
+ * s = amax / 448 and code = RNE_satfinite(x * (448 / amax)) (s = 1 when amax = 0); every scale stays inside one image:
+ *   Q: one scale per (token, head) over its 64 channels, K: one per (image, head) over all Lk tokens, V: one per (image, head,
+ *   channel) over all Lk tokens, P: codes RNE_satfinite_e4m3(2^8 p) with p = 2^(logit - running row max) in fp32.
+ * The row sum l adds the unrounded fp32 p; out[q, d] = acc[q, d] * sv[d] / (2^8 l), rounded once to bf16.
+ *
+ * supir_attention_quant_fp8: from bf16 q [B*Lq, ldq] and k, v [B*Lk, ldk / ldv] (head h at column h*64; column slices are
+ * fine, Lq may differ from Lk) writes q8 [B*Lq, ldq8] e4m3 with sq [B*Lq, H], k8 [B*Lk, ldk8] with sk [B, H], and vt8
+ * [B, H, 64, ld_vt]: V transposed (row (b, h, d) holds the keys of channel d), with the keys of every 32-key group permuted
+ * so that k position 16a + 4c + i holds key 16a + 2c + (i & 1) + 8 (i >> 1), and zeros from Lk to ld_vt; sv [B, H, 64].
+ * amax_ws: B * H * 65 unsigned ints of scratch (reset on the stream by the call). bf16 leading dims are multiples of 8, e4m3
+ * ones and ld_vt multiples of 16; ld_vt >= Lk; H <= 128; q, k, v, q8, k8, vt8 16-byte aligned. Three kernels and a memset.
+ *
+ * supir_attention_fp8: out [B*Lq, ldo] bf16 = softmax(Q K^T * scale) V from those operands. ldq, ldk, ld_vt multiples of 16,
+ * ldq, ldk >= H*64, ld_vt >= Lk, ldo a multiple of 8 and >= H*64, out 4-byte aligned. The split of the exponentials between
+ * MUFU.EX2 and the FMA-pipe polynomial is fixed at compile time: supir_set_attention_exp_emulation and
+ * supir_set_attention_alu_pack do not affect this kernel. */
+int supir_attention_quant_fp8(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* q8,
+                              long long ldq8, float* sq, void* k8, long long ldk8, float* sk, void* vt8, long long ld_vt, float* sv,
+                              unsigned int* amax_ws, int B, int H, int Lq, int Lk, void* stream);
+int supir_attention_fp8(const void* q8, long long ldq, const float* sq, const void* k8, long long ldk, const float* sk,
+                        const void* vt8, long long ld_vt, const float* sv, void* out, long long ldo, int B, int H, int Lq, int Lk,
+                        int head_dim, float scale, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------------ */
 /* K7/K8/K10/K12/K14 and data movement (elementwise.cu)                                                               */
 /* ------------------------------------------------------------------------------------------------------------------ */

@@ -53,6 +53,10 @@ _SIGS = {
     "supir_attention_1head_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_float, c_void_p],
     "supir_set_attention_exp_emulation": [c_int],
     "supir_set_attention_alu_pack": [c_int],
+    "supir_attention_quant_fp8": [c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p,
+                                  c_void_p, c_ll, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
+    "supir_attention_fp8": [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_int,
+                            c_int, c_int, c_int, c_float, c_void_p],
     "supir_upsample_nearest2x": [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p],
     "supir_im2col_3x3_s2": [c_void_p, c_ll, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "supir_copy2d_bf16": [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_int, c_void_p],

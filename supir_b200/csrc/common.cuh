@@ -294,4 +294,21 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return y;
 }
 
+// 2^x on the FMA / ALU pipes (no MUFU). x is clamped at -126 (result 2^-126 ~ 0 for anything below, including the -inf
+// of masked keys): Cody-Waite split x = n + f (round-down add of the 1.5*2^23 magic constant), degree-3 minimax
+// polynomial for 2^f on [0,1) (max rel. error 8.8e-5 = 2^-13.5, far below the bf16 rounding of P at 2^-9), exponent
+// reinserted with one integer shift-add.
+__device__ __forceinline__ float ex2_emulated(float x) {
+    const float kMagic = 12582912.0f;                       // 1.5 * 2^23: x + magic has ulp 1, floor(x) lands in the low mantissa bits
+    x = fmaxf(x, -126.0f);
+    const float xr = __fadd_rd(x, kMagic);                  // magic + floor(x)
+    const float xf = __fadd_rn(xr, -kMagic);                // floor(x), exact
+    const float fr = __fadd_rn(x, -xf);                     // x - floor(x) in [0, 1), exact
+    float p = fmaf(0.077119089663028717041015625f, fr, 0.227564394474029541015625f);
+    p = fmaf(p, fr, 0.695146143436431884765625f);
+    p = fmaf(p, fr, 1.0f);                                  // 2^f in [1, 2]
+    // bits(magic + n) = 0x4B400000 + n: the low 9 bits of the constant are zero, so << 23 leaves n in the exponent field
+    return __uint_as_float(__float_as_uint(p) + (__float_as_uint(xr) << 23));
+}
+
 }  // namespace supir

@@ -27,6 +27,12 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
     return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 
+// the same with 64-byte swizzle (TMA SWIZZLE_64B, layout 2): K-major tile of 64-byte rows, SBO = 512 (8 rows). The tile
+// must start on a 512-byte boundary (one swizzle period); a k-step inside the row advances the start address.
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) | ((uint64_t)2 << 62);
+}
+
 // D (+)= A[smem] * B[smem]^T, both K-major (the only layout e4m3 operands support)
 #define SUPIR_WGMMA_SS_N64(KTY, TRANS) \
     asm volatile( \
@@ -100,5 +106,16 @@ __device__ __forceinline__ void wgmma_rs_n64_tb(float (&d)[32], const uint32_t (
     else SUPIR_WGMMA_RS_N64_TB(".bf16.bf16");
 }
 #undef SUPIR_WGMMA_RS_N64_TB
+
+// D (+)= A[registers, m64k32 e4m3 fragment] * B[smem]^T, B K-major. A fragment (thread lane l of warp w, c = l % 4): register
+// 0 holds row 16 w + l / 4, k 4c..4c+3 (first k in the low byte); register 1 the same k of row + 8; registers 2, 3 the same
+// for k 16 + 4c..19 + 4c.
+__device__ __forceinline__ void wgmma_rs_n64_e4m3(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, int scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
+}
 
 }  // namespace supir

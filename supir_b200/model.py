@@ -26,7 +26,8 @@ def _get(cfg, key, default=None):
 class SUPIRModel(nn.Module):
     def __init__(self, control_stage_config, network_config, denoiser_config, first_stage_config, conditioner_config=None,
                  sampler_config=None, network_wrapper=None, ae_dtype="fp32", diffusion_dtype="fp32", scale_factor=1.0,
-                 p_p="", n_p="", disable_first_stage_autocast=False, fp8_convs=False, **unused):
+                 p_p="", n_p="", disable_first_stage_autocast=False, fp8_convs=False, fp8_attention=False,
+                 **unused):
         super().__init__()
         wrapper_cls = get_obj_from_str(network_wrapper or "sgm.modules.diffusionmodules.wrappers.ControlWrapper")
         self.model = wrapper_cls(instantiate_from_config(network_config))
@@ -56,6 +57,10 @@ class SUPIRModel(nn.Module):
         assert not fp8_convs or diffusion_dtype == "fp8", "fp8_convs needs diffusion_dtype='fp8'"
         if fp8_convs:
             self.model.fp8_convs = True
+        # fp8_attention: in the "fp8" mode, the self-attentions and ZeroCrossAttn on e4m3 tensor cores as well
+        assert not fp8_attention or diffusion_dtype == "fp8", "fp8_attention needs diffusion_dtype='fp8'"
+        if fp8_attention:
+            self.model.fp8_attention = True
         self.p_p, self.n_p = p_p, n_p
         self._shard_group, self._shard = None, False
 

@@ -8,7 +8,8 @@ gamma|beta matrices, fp32 biases) and `run()` issues hand-written sm_90a kernels
 channels-last activations of that dtype (torch.autocast(bfloat16) or autocast(float16) numerics). `pack(float8_e4m3fn)` is
 the bf16 pack except for the Linear layers inside every BasicTransformerBlock, which hold e4m3 weights with per-row scales and
 run on FP8 tensor cores (see `linear`); `pack(float8_e4m3fn, fp8_convs=True)` also runs the two 3x3 convolutions of every
-ResBlock on them (see `ResBlock.run`). Options the SUPIR configs never use raise NotImplementedError.
+ResBlock on them (see `ResBlock.run`), and `fp8_attention=True` the self-attentions and ZeroCrossAttn (see `attention`).
+Options the SUPIR configs never use raise NotImplementedError.
 """
 import os
 
@@ -98,6 +99,23 @@ def linear(ctx, x, w, out, **kw):
     ops.quantize_rows(x, q, sc)
     ops.gemm_fp8(q, sc, *w, out, **kw)
     ctx.pool.put(q, sc)
+    return out
+
+
+def attention(ctx, fp8, q, k, v, out, B, heads, Lq, Lk):
+    """softmax(q k^T / 8) v per head into `out`: the 16-bit kernel (ops.attention), or with `fp8` (the fp8_attention option)
+    the operand pass (ops.attention_quant_fp8: e4m3 codes and scales of q, k and transposed v) and the e4m3 kernel
+    (ops.attention_fp8)."""
+    if not fp8:
+        return ops.attention(q, k, v, out, B, heads, Lq, Lk)
+    get, f32 = ctx.pool.get, torch.float32
+    q8, k8 = ctx.new(B * Lq, heads * 64, ops.FP8), ctx.new(B * Lk, heads * 64, ops.FP8)
+    vt8 = get((B, heads, 64, ops.attention_vt_ld(Lk)), ops.FP8)
+    sq, sk, sv = get((B * Lq, heads), f32), get((B, heads), f32), get((B, heads, 64), f32)
+    amax = get((B * heads * 65,), torch.int32)
+    ops.attention_quant_fp8(q, k, v, B, heads, Lq, Lk, q8, sq, k8, sk, vt8, sv, amax)
+    ops.attention_fp8(q8, sq, k8, sk, vt8, sv, out, B, heads, Lq, Lk)
+    ctx.pool.put(q8, k8, vt8, sq, sk, sv, amax)
     return out
 
 
@@ -296,6 +314,7 @@ class CrossAttention(nn.Module):
 
     _ln = None      # (gamma, beta) of the LayerNorm in front of the query projection, set by BasicTransformerBlock.pack
     _fp8 = False    # FP8 query / QKV and output projections, set by BasicTransformerBlock.pack
+    fp8_attention = False   # softmax(QK^T)V on e4m3 operands, set by the network's pack(float8_e4m3fn, fp8_attention=True)
 
     def pack(self, dtype=BF16):
         if self._fp8:
@@ -337,7 +356,7 @@ class CrossAttention(nn.Module):
         qkv = ctx.new(B * L, 3 * C)
         linear(ctx, xn, self._wqkv, qkv, **self._ln_args(stats))
         a = ctx.new(B * L, C)
-        ops.attention(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], a, B, self.heads, L, L)
+        attention(ctx, self.fp8_attention, qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], a, B, self.heads, L, L)
         ctx.free(qkv)
         out = ctx.new(B * L, x_res.shape[1])
         linear(ctx, a, self._wo, out, bias=self._bo, residual=x_res)
@@ -349,7 +368,7 @@ class CrossAttention(nn.Module):
         q = ctx.new(B * L, C)
         linear(ctx, xn, self._wq, q, **self._ln_args(stats))
         a = ctx.new(B * L, C)
-        ops.attention(q, k, v, a, B, self.heads, L, Lk)
+        attention(ctx, self.fp8_attention, q, k, v, a, B, self.heads, L, Lk)
         ctx.free(q)
         out = ctx.new(B * L, self.to_out[0].out_features)
         linear(ctx, a, self._wo, out, bias=self._bo, residual=x_res if residual else None)
@@ -629,18 +648,22 @@ class _UNetBase(nn.Module):
         return chans, ch, ds, ted, transformer_depth, st
 
     # ---- packing -----------------------------------------------------------------------------------------------------
-    def pack(self, dtype=BF16, fp8_convs=False):
+    def pack(self, dtype=BF16, fp8_convs=False, fp8_attention=False):
         """Convert parameters into kernel layouts (call again after load_state_dict / .to()). `dtype` is the compute dtype:
         torch.bfloat16, or torch.float16 for the fp16 mode (every 16-bit weight, bias value and activation in fp16), or
         torch.float8_e4m3fn for the FP8 mode: bf16 everywhere except the Linear layers of every BasicTransformerBlock (QKV,
         to_out, the cross-attention's to_q, GEGLU, ff.net.2), which hold e4m3 weights with one fp32 scale per output channel
         and take e4m3 activations with one scale per row. `fp8_convs` (FP8 mode only) also runs the two 3x3 convolutions of
         every ResBlock (in_layers.2, out_layers.3) on e4m3 weights with one scale per output channel and e4m3 activations with
-        one scale per image (the GroupNorm + SiLU in front of them writes them)."""
+        one scale per image (the GroupNorm + SiLU in front of them writes them). `fp8_attention` (FP8 mode only) runs the
+        self-attention of every BasicTransformerBlock and the attention of every ZeroCrossAttn on e4m3 operands (`attention`);
+        the text cross-attention (attn2) stays bf16."""
         if dtype not in (BF16, ops.F16, ops.FP8):
             raise ValueError(f"compute dtype {dtype} is not supported (bfloat16, float16 or float8_e4m3fn)")
         if fp8_convs and dtype != ops.FP8:
             raise ValueError(f"fp8_convs needs the float8_e4m3fn compute dtype (got {dtype})")
+        if fp8_attention and dtype != ops.FP8:
+            raise ValueError(f"fp8_attention needs the float8_e4m3fn compute dtype (got {dtype})")
         fp8 = dtype == ops.FP8
         dtype = BF16 if fp8 else dtype
         res, xattn = [], []
@@ -651,6 +674,9 @@ class _UNetBase(nn.Module):
             if isinstance(m, BasicTransformerBlock):
                 xattn.append(m.attn2)
                 m.fp8 = fp8
+                m.attn1.fp8_attention = bool(fp8_attention)
+            if isinstance(m, ZeroCrossAttn):
+                m.attn.fp8_attention = bool(fp8_attention)
         off = 0
         for r in res:
             r.emb_offset = off
@@ -676,6 +702,7 @@ class _UNetBase(nn.Module):
         self._packed_dtype = dtype
         self._fp8_linears = fp8
         self._fp8_convs = bool(fp8_convs)
+        self._fp8_attention = bool(fp8_attention)
         return self
 
     def project_context(self, context_16, out):
@@ -784,8 +811,8 @@ class LightGLVUNet(_UNetBase):
         for i in [6, 3]:
             self.project_modules.insert(i, ZeroCrossAttn(cond_output_channels[i], concat_channels[i]))
 
-    def pack(self, dtype=BF16, fp8_convs=False):
-        super().pack(dtype, fp8_convs)
+    def pack(self, dtype=BF16, fp8_convs=False, fp8_attention=False):
+        super().pack(dtype, fp8_convs, fp8_attention)
         dtype = self._packed_dtype
         pack_norm(self.out[0])
         w = self.out[2].weight.detach()

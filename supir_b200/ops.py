@@ -10,7 +10,9 @@ The ops the diffusion networks use also take fp16 operands (their fp16 compute m
 FP8 linear layers (the networks' float8_e4m3fn mode): gemm_fp8 multiplies e4m3 operands with one fp32 scale per row of each
 (quantize_weight at pack time; quantize_rows / layernorm_quant for the activations) into a bf16 result. FP8 convolutions (the
 fp8_convs option of that mode): conv3x3_fp8 takes e4m3 activations with one scale per image (groupnorm_apply_quant) and e4m3
-weights with one scale per output channel (quantize_weight of the packed [Cout, 9*Cin] matrix).
+weights with one scale per output channel (quantize_weight of the packed [Cout, 9*Cin] matrix). FP8 attention (the
+fp8_attention option): attention_quant_fp8 writes e4m3 Q / K / transposed V and their scales from bf16 q, k, v, and
+attention_fp8 runs softmax(Q K^T / 8) V on them into a bf16 result.
 """
 import ctypes
 
@@ -300,6 +302,66 @@ def attention(q, k, v, out, B, heads, Lq, Lk, scale=None):
     d = q.shape[1] // heads
     call(name, _ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(out),
          out.stride(0), B, heads, Lq, Lk, d, float(scale if scale is not None else d ** -0.5), _stream())
+    return out
+
+
+def attention_vt_ld(Lk):
+    """Row length of attention_quant_fp8's transposed V codes: Lk rounded up to a multiple of 16 bytes."""
+    return -(-int(Lk) // 16) * 16
+
+
+def attention_quant_fp8(q, k, v, B, heads, Lq, Lk, q8, sq, k8, sk, vt8, sv, amax_ws):
+    """attention_fp8's operands from bf16 q [B*Lq, >= heads*64] and k, v [B*Lk, ...] (column slices are fine; see
+    supir_attention_quant_fp8): q8 (e4m3, q's shape) with sq fp32 [B*Lq, heads] per (token, head); k8 (k's shape) with sk
+    [B, heads] per (image, head); vt8 e4m3 [B, heads, 64, attention_vt_ld(Lk)] (V transposed, keys permuted inside every group
+    of 32, zero padded) with sv [B, heads, 64] per (image, head, channel). amax_ws: int32 [B * heads * 65] scratch."""
+    if q.dtype != BF16 or k.dtype != BF16 or v.dtype != BF16:
+        raise TypeError(f"attention_quant_fp8: q, k, v are bfloat16 (got {q.dtype}, {k.dtype}, {v.dtype})")
+    if q8.dtype != FP8 or k8.dtype != FP8 or vt8.dtype != FP8:
+        raise TypeError("attention_quant_fp8: q8, k8, vt8 are float8_e4m3fn")
+    if sq.dtype != torch.float32 or sk.dtype != torch.float32 or sv.dtype != torch.float32 or amax_ws.dtype != torch.int32:
+        raise TypeError("attention_quant_fp8: scales are float32, amax_ws int32")
+    _need_cuda(q, k, v, q8, sq, k8, sk, vt8, sv, amax_ws)
+    for t in (q, k, v):
+        _mat(t)
+    _mat(q8, FP8), _mat(k8, FP8)
+    C = heads * 64
+    assert q.shape == (B * Lq, C) and k.shape == (B * Lk, C) and v.shape == (B * Lk, C), (q.shape, k.shape, v.shape)
+    assert q8.shape == q.shape and k8.shape == k.shape, (q8.shape, k8.shape)
+    ld_vt = _vt_ld(vt8, B, heads, Lk)
+    assert sq.shape == (B * Lq, heads) and sk.shape == (B, heads) and sv.shape == (B, heads, 64) and amax_ws.shape == (B * heads * 65,)
+    assert sq.is_contiguous() and sk.is_contiguous() and sv.is_contiguous() and amax_ws.is_contiguous()
+    call("supir_attention_quant_fp8", _ptr(q), q.stride(0), _ptr(k), k.stride(0), _ptr(v), v.stride(0), _ptr(q8), q8.stride(0),
+         _ptr(sq), _ptr(k8), k8.stride(0), _ptr(sk), _ptr(vt8), ld_vt, _ptr(sv), _ptr(amax_ws), B, heads, Lq, Lk, _stream())
+    return q8, sq, k8, sk, vt8, sv
+
+
+def _vt_ld(vt8, B, heads, Lk):
+    """Row stride of a [B, heads, 64, >= Lk] transposed-V tensor whose rows are evenly spaced."""
+    assert vt8.dim() == 4 and vt8.shape[:3] == (B, heads, 64) and vt8.shape[3] >= Lk and vt8.stride(3) == 1, (vt8.shape, vt8.stride())
+    ld = vt8.stride(2)
+    assert vt8.stride(1) == 64 * ld and vt8.stride(0) == heads * 64 * ld and ld >= vt8.shape[3], (vt8.shape, vt8.stride())
+    return ld
+
+
+def attention_fp8(q8, sq, k8, sk, vt8, sv, out, B, heads, Lq, Lk, scale=None):
+    """out [B*Lq, >= heads*64] bf16 = softmax(Q K^T * scale) V on e4m3 tensor cores from attention_quant_fp8's operands
+    (supir_attention_fp8; head_dim 64, scale defaults to 64^-0.5)."""
+    if q8.dtype != FP8 or k8.dtype != FP8 or vt8.dtype != FP8:
+        raise TypeError(f"attention_fp8: operands are float8_e4m3fn (got {q8.dtype}, {k8.dtype}, {vt8.dtype})")
+    if sq.dtype != torch.float32 or sk.dtype != torch.float32 or sv.dtype != torch.float32:
+        raise TypeError("attention_fp8: scales are float32")
+    if out.dtype != BF16:
+        raise TypeError(f"attention_fp8: out is bfloat16 (got {out.dtype})")
+    _need_cuda(q8, sq, k8, sk, vt8, sv, out)
+    _mat(q8, FP8), _mat(k8, FP8), _mat(out)
+    C = heads * 64
+    assert q8.shape == (B * Lq, C) and k8.shape == (B * Lk, C) and out.shape == (B * Lq, C), (q8.shape, k8.shape, out.shape)
+    ld_vt = _vt_ld(vt8, B, heads, Lk)
+    assert sq.shape == (B * Lq, heads) and sk.shape == (B, heads) and sv.shape == (B, heads, 64)
+    assert sq.is_contiguous() and sk.is_contiguous() and sv.is_contiguous()
+    call("supir_attention_fp8", _ptr(q8), q8.stride(0), _ptr(sq), _ptr(k8), k8.stride(0), _ptr(sk), _ptr(vt8), ld_vt, _ptr(sv),
+         _ptr(out), out.stride(0), B, heads, Lq, Lk, 64, float(scale if scale is not None else 0.125), _stream())
     return out
 
 

@@ -8,7 +8,8 @@ static input/output buffers, so the ~2000 kernel launches of a denoiser call cos
 `.dtype` selects the compute dtype of both networks: torch.float16 runs them in fp16 (torch.autocast(float16) numerics, the
 reference's default `diffusion_dtype`), torch.bfloat16 in bf16, torch.float8_e4m3fn in bf16 with the transformer blocks'
 Linear layers on FP8 tensor cores (nets.py); any other value (fp32) warns and computes bf16. `.fp8_convs = True` (FP8 dtype
-only, default False) also runs the ResBlocks' 3x3 convolutions on FP8 tensor cores.
+only, default False) also runs the ResBlocks' 3x3 convolutions on FP8 tensor cores, and `.fp8_attention = True` (FP8 dtype
+only, default False, independent of fp8_convs) the self-attentions and ZeroCrossAttn.
 """
 import os
 import warnings
@@ -94,6 +95,7 @@ class ControlWrapper(nn.Module):
         self.replayed_launches = 0      # kernels launched through CUDA-graph replays (supir_launch_count() sees eager ones)
         self.dtype = dtype
         self.fp8_convs = False
+        self.fp8_attention = False
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate())
 
     @staticmethod
@@ -133,6 +135,20 @@ class ControlWrapper(nn.Module):
             self.invalidate()           # packed weights and captured graphs are in the old mode: drop them
 
     @property
+    def fp8_attention(self):
+        """FP8 mode option: the self-attention of every transformer block and the attention of every ZeroCrossAttn run on e4m3
+        operands (nets.attention); the text cross-attention stays bf16. Part of the pack mode: packing with it under another
+        dtype raises."""
+        return self._fp8_attention
+
+    @fp8_attention.setter
+    def fp8_attention(self, value):
+        old = getattr(self, "_fp8_attention", None)
+        self._fp8_attention = bool(value)
+        if old is not None and old != self._fp8_attention:
+            self.invalidate()           # packed weights and captured graphs are in the old mode: drop them
+
+    @property
     def compute_dtype(self):
         return self._compute_dtype(self._dtype)
 
@@ -155,8 +171,8 @@ class ControlWrapper(nn.Module):
         return r
 
     def pack(self):
-        self.diffusion_model.pack(self._pack_mode(self._dtype), fp8_convs=self._fp8_convs)
-        self.control_model.pack(self._pack_mode(self._dtype), fp8_convs=self._fp8_convs)
+        for net in (self.diffusion_model, self.control_model):
+            net.pack(self._pack_mode(self._dtype), fp8_convs=self._fp8_convs, fp8_attention=self._fp8_attention)
         self._packed = True
         return self
 

@@ -1,13 +1,15 @@
-"""python tools/bench_fp8.py [--out DIR] : bf16 against the FP8 linears mode (ControlWrapper.dtype = torch.float8_e4m3fn) and the
-FP8 linears + convs mode (also ControlWrapper.fp8_convs = True) on the bench's networks (SUPIR-v0 + SDXL-base shapes, random
-weights), in one process:
+"""python tools/bench_fp8.py [--out DIR] : bf16 against the FP8 modes on the bench's networks (SUPIR-v0 + SDXL-base shapes, random
+weights), in one process. Modes: the FP8 linears (ControlWrapper.dtype = torch.float8_e4m3fn), + convs (.fp8_convs = True),
++ attention (.fp8_attention = True), + convs + attention.
 
-  1. one denoiser call of the bench plan (34 rows = 17 windows x CFG pair of 128^2 latent), bf16 / FP8 / FP8 + convs alternated
-     3x each, CUDA events around 5 graph replays per window, with the card, its power limit and the median SM clock of each window;
-  2. the per-launch shape table of one eager call in each mode (the SUPIR_BENCH_DUMP_SHAPES form of bench.py), GEMM-class
-     launches (gemm, gemm_fp8, conv3x3, conv3x3_fp8), the quantization passes (layernorm_quant, quantize_rows) and the GroupNorm
-     applies (groupnorm_apply, groupnorm_apply_quant) each timed with a CUDA-event pair;
-  3. the cfg3 EDM step (49 windows, tile batch 17) in the three modes, alternated, without the VAE (a random latent);
+  1. one denoiser call of the bench plan (34 rows = 17 windows x CFG pair of 128^2 latent), the modes alternated 3x each (--windows), CUDA
+     events around 5 graph replays per window, with the card, its power limit and the median SM clock of each window; the same
+     for one untiled CFG-pair call of a 256^2 latent (2 rows, the shape of the cfg2 workload);
+  2. the per-launch shape table of one eager call in each mode and shape (the SUPIR_BENCH_DUMP_SHAPES form of bench.py),
+     GEMM-class launches (gemm, gemm_fp8, conv3x3, conv3x3_fp8), the attentions (attention, attention_fp8 and its operand pass
+     attention_quant_fp8), the quantization passes (layernorm_quant, quantize_rows) and the GroupNorm applies (groupnorm_apply,
+     groupnorm_apply_quant) each timed with a CUDA-event pair;
+  3. the cfg3 EDM step (49 windows, tile batch 17) in every mode, alternated, without the VAE (a random latent);
   4. the resident bytes of the packed networks in each mode.
 
 Prints one JSON line and writes it (and the shape table) under --out. Reuses bench.engine_config / ClockSampler unchanged."""
@@ -26,7 +28,9 @@ sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 
 FP8, BF = torch.float8_e4m3fn, torch.bfloat16
-MODES = {"bf16": (BF, False), "fp8": (FP8, False), "fp8_convs": (FP8, True)}     # (ControlWrapper.dtype, .fp8_convs)
+# (ControlWrapper.dtype, .fp8_convs, .fp8_attention)
+MODES = {"bf16": (BF, False, False), "fp8": (FP8, False, False), "fp8_convs": (FP8, True, False), "fp8_attn": (FP8, False, True),
+         "fp8_convs_attn": (FP8, True, True)}
 
 
 def card():
@@ -50,9 +54,16 @@ def packed_bytes(net):
 
 
 def set_mode(net, mode):
-    net.dtype, net.fp8_convs = MODES[mode]
+    net.dtype, net.fp8_convs, net.fp8_attention = MODES[mode]
     net.pack()
     torch.cuda.empty_cache()
+
+
+def call_inputs(B, side):
+    x = torch.randn(B, 4, side, side, device="cuda")
+    cond = {"crossattn": torch.randn(B, 77, 2048, device="cuda"), "vector": torch.randn(B, 2816, device="cuda"),
+            "control": torch.randn(B, 4, side, side, device="cuda")}
+    return x, torch.full((B,), 500.0, device="cuda"), cond
 
 
 def time_call(net, args, reps):
@@ -102,6 +113,12 @@ def shape_table(net):
     wrap("layernorm_quant", lambda x, g, b, q, s, eps=1e-5: (0.0, ("layernorm_quant", x.shape[0], 0, x.shape[1], 0), 3))
     wrap("groupnorm_apply", lambda x, B, HW, out, *a, **kw: (0.0, ("groupnorm_apply", x.shape[0], 0, x.shape[1], 0), 4))
     wrap("groupnorm_apply_quant", lambda x, B, HW, *a, **kw: (0.0, ("groupnorm_apply_quant", x.shape[0], 0, x.shape[1], 0), 5))
+    # attentions: M = B * Lq, N = Lk, K = heads * 64, 4 M N K flop (Q K^T and P V); the operand pass as bf16 q, k, v read + k, v
+    # read again by the amax pass + e4m3 written: 2 (Lq + 4 Lk) + Lq + 2 Lk bytes per (row, column) of M x K, taken as Lq = Lk
+    wrap("attention", lambda q, k, v, out, B, heads, Lq, Lk, **kw: (4.0 * B * Lq * Lk * heads * 64, ("attention", B * Lq, Lk, heads * 64, 0)))
+    wrap("attention_fp8", lambda q8, sq, k8, sk, vt8, sv, out, B, heads, Lq, Lk, **kw: (4.0 * B * Lq * Lk * heads * 64,
+                                                                                        ("attention_fp8", B * Lq, Lk, heads * 64, 0)))
+    wrap("attention_quant_fp8", lambda q, k, v, B, heads, Lq, Lk, *a, **kw: (0.0, ("attention_quant_fp8", B * Lq, Lk, heads * 64, 0), 13))
     plan = next(iter(net._plans.values()))
     try:
         plan._run()
@@ -127,30 +144,30 @@ def main():
     ap.add_argument("--out", default=tempfile.gettempdir(), help="directory for bench_fp8.json (default: the temporary directory)")
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--steps", type=int, default=2)
+    ap.add_argument("--windows", type=int, default=3, help="times every mode is timed, alternated with the others")
     args = ap.parse_args()
     torch.manual_seed(1234)
     res = {"card": card()}
     w = bench.WORKLOADS["cfg3"]
     m = bench.build_engine(w, "cuda:0", 1)
     net = m.model
-    # ---- 1. one 34-row denoiser call of 128^2 latent ----
-    B = 34
-    x = torch.randn(B, 4, 128, 128, device="cuda")
-    cond = {"crossattn": torch.randn(B, 77, 2048, device="cuda"), "vector": torch.randn(B, 2816, device="cuda"),
-            "control": torch.randn(B, 4, 128, 128, device="cuda")}
-    t = torch.full((B,), 500.0, device="cuda")
-    call_args = (x, t, cond)
-    calls = {mode: [] for mode in MODES}
+    # ---- 1. one 34-row denoiser call of 128^2 latent (tiled cfg3), one 2-row call of 256^2 latent (untiled cfg2) ----
     res["resident_bytes"] = {}
-    for rep in range(3):
-        for mode in MODES:
-            set_mode(net, mode)
-            res["resident_bytes"][mode] = packed_bytes(net)
-            ms, clk = time_call(net, call_args, args.reps)
-            calls[mode].append({"ms": ms, "sm_mhz": clk.get("sm_mhz"), "reasons": clk.get("reasons")})
-            if rep == 2:
-                res[f"{mode}_shape_table"] = shape_table(net)
-    res["call_34rows_128"] = {k: {"median_ms": float(np.median([c["ms"] for c in v])), "windows": v} for k, v in calls.items()}
+    for key, (B, side) in (("call_34rows_128", (34, 128)), ("call_2rows_256", (2, 256))):
+        call_args = call_inputs(B, side)
+        calls = {mode: [] for mode in MODES}
+        for rep in range(args.windows):
+            for mode in MODES:
+                set_mode(net, mode)
+                res["resident_bytes"][mode] = packed_bytes(net)
+                ms, clk = time_call(net, call_args, args.reps)
+                calls[mode].append({"ms": ms, "sm_mhz": clk.get("sm_mhz"), "reasons": clk.get("reasons")})
+                if rep == args.windows - 1:
+                    res[f"{mode}_shape_table" + ("" if side == 128 else "_256")] = shape_table(net)
+        res[key] = {k: {"median_ms": float(np.median([c["ms"] for c in v])), "windows": v} for k, v in calls.items()}
+        del call_args
+        net.clear_plans()
+        torch.cuda.empty_cache()
     # ---- 3. the cfg3 EDM step (no VAE: a random latent) ----
     from supir_b200 import sampling
     latent = w["in_px"] * w["upscale"] // 8
@@ -158,7 +175,7 @@ def main():
     uc = {"crossattn": torch.randn(1, 77, 2048, device="cuda"), "vector": torch.randn(1, 2816, device="cuda")}
     z = 0.5 * torch.randn(1, 4, latent, latent, device="cuda")
     steps = {mode: [] for mode in MODES}
-    for rep in range(3):
+    for rep in range(args.windows):
         for mode in MODES:
             set_mode(net, mode)
             smp = m.make_sampler(w["steps"], -1.0, 5, 1.01, 4.0, True, 1.0)
@@ -187,7 +204,7 @@ def main():
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "bench_fp8.json"), "w") as f:
         json.dump(res, f, indent=1)
-    short = {k: v for k, v in res.items() if not k.endswith("shape_table")}
+    short = {k: v for k, v in res.items() if "shape_table" not in k}
     short["fp8_shape_table_top"] = res["fp8_shape_table"]["rows"][:12]
     short["fp8_convs_shape_table_top"] = res["fp8_convs_shape_table"]["rows"][:12]
     # the per-launch rows the convs option changes: 3x3 convolutions and GroupNorm applies, before (fp8) and after (fp8_convs)
@@ -196,6 +213,12 @@ def main():
         t = res[f"{mode}_shape_table"]["rows"]
         short[f"{mode}_conv_rows"] = [r for r in t if r["op"] in conv_ops]
         short[f"{mode}_ms_by_op"] = {op: round(sum(r["ms"] for r in t if r["op"] == op), 3) for op in sorted({r["op"] for r in t})}
+    # the per-launch rows the attention option changes, at both shapes and in every mode
+    attn_ops = ("attention", "attention_fp8", "attention_quant_fp8")
+    for mode in MODES:
+        for suffix in ("", "_256"):
+            t = res[f"{mode}_shape_table{suffix}"]["rows"]
+            short[f"{mode}_attention_rows{suffix}"] = [r for r in t if r["op"] in attn_ops]
     print(json.dumps(short))
 
 

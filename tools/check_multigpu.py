@@ -1,7 +1,8 @@
-"""torchrun --nproc-per-node N tools/check_multigpu.py [--dtype bf16|fp16|fp8] [--fp8-convs] : the unit-sharded tiled sampler and the
+"""torchrun --nproc-per-node N tools/check_multigpu.py [--dtype bf16|fp16|fp8] [--fp8-convs] [--fp8-attention] : the unit-sharded tiled sampler and the
 tile-sharded VAE give the same result as the single-GPU path, bit for bit, on every rank (also run by tests/test_gpu_multigpu.py and,
 with --dtype fp16 / fp8 / --fp8-convs, by tests/test_gpu_fp16.py / test_gpu_fp8.py / test_gpu_fp8_conv.py when >= 2 GPUs). --dtype
-is the compute dtype of the diffusion networks; --fp8-convs (implies --dtype fp8) also runs the ResBlocks' 3x3 convolutions in FP8."""
+is the compute dtype of the diffusion networks; --fp8-convs (implies --dtype fp8) also runs the ResBlocks' 3x3 convolutions in FP8,
+--fp8-attention (implies --dtype fp8) the self-attentions and ZeroCrossAttn."""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -21,10 +22,10 @@ def main():
     with torch.device("meta"):
         unet = nets.LightGLVUNet(mode="XL-base", project_type="ZeroSFT", project_channel_scale=2, **cfg)
         ctrl = nets.GLVControl(input_upscale=1, **cfg)
-    fp8_convs = "--fp8-convs" in sys.argv
-    dname = sys.argv[sys.argv.index("--dtype") + 1] if "--dtype" in sys.argv else ("fp8" if fp8_convs else "bf16")
+    fp8_convs, fp8_attention = "--fp8-convs" in sys.argv, "--fp8-attention" in sys.argv
+    dname = sys.argv[sys.argv.index("--dtype") + 1] if "--dtype" in sys.argv else ("fp8" if fp8_convs or fp8_attention else "bf16")
     net = wrappers.ControlWrapper(unet, dtype={"bf16": torch.bfloat16, "fp16": torch.float16, "fp8": torch.float8_e4m3fn}[dname])
-    net.fp8_convs = fp8_convs
+    net.fp8_convs, net.fp8_attention = fp8_convs, fp8_attention
     net.load_control_model(ctrl)
     net.to_empty(device="cuda")
     net.load_state_dict(sd)
@@ -72,7 +73,7 @@ def main():
     ref = torch.from_numpy(gv["dec_tiled"]).cuda()
     rel = float((d_sharded - ref).norm() / ref.norm())
     if rank == 0:
-        print(json.dumps({"world": world, "dtype": dname, "fp8_convs": fp8_convs, "sampler_sharded_equals_single": same, "untiled_branch_parallel_equals_single": pair_same, "identical_on_all_ranks": same_ranks,
+        print(json.dumps({"world": world, "dtype": dname, "fp8_convs": fp8_convs, "fp8_attention": fp8_attention, "sampler_sharded_equals_single": same, "untiled_branch_parallel_equals_single": pair_same, "identical_on_all_ranks": same_ranks,
                           "vae_sharded_rel_fro_vs_reference": rel, "vae_sharded_equals_single": vae_same, "finite": bool(torch.isfinite(a).all())}))
     dist.barrier()
     dist.destroy_process_group()
