@@ -174,24 +174,96 @@ __device__ __forceinline__ EpiRow epi_row(const GemmKernelParams& p, int mt, int
     return r;
 }
 
+// This thread's columns of a fragment as pairs: s[j] = (src[n], src[n + 1]) for n = n0 + 8 j (n0 even), all at fixed offsets
+// from one address. One 64-bit load per pair when every column is inside N (`full`) and `src` is 8-byte aligned; otherwise
+// two 32-bit loads, and columns past N read as 0 (their results are never stored).
+template <int NJ>
+__device__ __forceinline__ void load_col_pairs(float2 (&s)[NJ], const float* src, int n0, int N, bool full) {
+    if (full && (reinterpret_cast<uintptr_t>(src) & 7) == 0) {
+        const float2* q = reinterpret_cast<const float2*>(src + n0);
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) s[j] = __ldg(q + 4 * j);
+    } else {
+        const float* q = src + n0;
+#pragma unroll
+        for (int j = 0; j < NJ; ++j)
+            s[j] = make_float2(n0 + 8 * j < N ? __ldg(q + 8 * j) : 0.f, n0 + 8 * j + 1 < N ? __ldg(q + 8 * j + 1) : 0.f);
+    }
+}
+
+// f(j, pair j) for every column pair j < NJ of this thread: one branch-free pass that issues all of its loads before the
+// first use
+template <int NJ, class F>
+__device__ __forceinline__ void col_pass(const float* src, int n0, int N, bool full, F&& f) {
+    float2 s[NJ];
+    load_col_pairs(s, src, n0, N, full);
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) f(j, s[j]);
+}
+
 // Epilogue of one m64 accumulator fragment of tile (mt, nt): rows [row0, row0 + 64) of the tile, of which this thread holds
-// rows row0 + r_lo and row0 + r_lo + 8, columns 8 j + cq (+1). STAGED: the residual is read from, and the output written to,
-// the fragment's staging buffer at shared address `frag` (stage_off layout; the residual was put there by TMA), and TMA stores
-// it afterwards; rows and columns outside the output are skipped here and clipped by the store. Otherwise both go straight
-// to global memory. The arithmetic and its rounding points are the same either way.
+// rows row0 + r_lo and row0 + r_lo + 8 (h = 0, 1: v[4 j + 2 h + e]), columns 8 j + cq + e. STAGED: the residual is read
+// from, and the output written to, the fragment's staging buffer at shared address `frag` (stage_off layout; the residual was
+// put there by TMA), and TMA stores it afterwards; rows and columns outside the output are skipped here and clipped by the
+// store. Otherwise both go straight to global memory. The arithmetic and its rounding points are the same either way.
+// The epilogue works on the accumulators in place (a copy would not fit in registers beside them: the next tile's wgmma
+// keeps them live, and overwrites them). Both rows share their columns, so each column operand is loaded once per fragment,
+// as pairs, in one branch-free pass (col_pass) applied to both rows; the per-row terms are loaded once per row.
 template <int BN, bool STAGED, class E>
-__device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const float (&acc)[BN / 2], int mt, int nt, int row0,
+__device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, float (&v)[BN / 2], int mt, int nt, int row0,
                                              int r_lo, int cq, uint32_t frag) {
+    constexpr int NJ = BN / 8;
+    const EpiRow row[2] = {epi_row(p, mt, row0 + r_lo), epi_row(p, mt, row0 + r_lo + 8)};
+    if (!row[0].ok && !row[1].ok) return;
+    const int n0 = nt * BN + cq;
+    const bool full = nt * BN + BN <= p.N;                    // every column of the tile is inside N
+    // Per-row terms. A row outside the output borrows the other row's (its results are never stored).
+    float sa[2] = {1.f, 1.f};
+    float2 st[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+    const float* rv[2] = {nullptr, nullptr};
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-        const int r = r_lo + 8 * h;
-        const EpiRow row = epi_row(p, mt, row0 + r);
-        if (!row.ok) continue;
-        const long long grow = row.grow;
-        const float* rv = p.rowvec ? p.rowvec + (long long)row.batch * p.rowvec_ld : nullptr;
+        const EpiRow rw = row[h].ok ? row[h] : row[h ^ 1];
         // E4m3: the accumulator times a_scale[row] * w_scale[column] comes first (sa * w_scale[n] below); a convolution's
         // activation scale is per image (a pixel's k-sum spans 9 input pixels: only a scale they share factors out of it)
-        const float sa = E::kFp8 ? __ldg(p.a_scale + (p.conv ? (long long)row.batch : grow)) : 1.f;
+        if constexpr (E::kFp8) sa[h] = __ldg(p.a_scale + (p.conv ? (long long)rw.batch : rw.grow));
+        if (p.ln_stats) st[h] = __ldg(p.ln_stats + rw.grow);
+        if (p.rowvec) rv[h] = p.rowvec + (long long)rw.batch * p.rowvec_ld;
+    }
+    // One pass per column operand (run-time branches: they keep the passes' loads apart)
+    if (E::kFp8 && p.w_scale)
+        col_pass<NJ>(p.w_scale, n0, p.N, full, [&](int j, float2 s) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) { v[4 * j + 2 * h] *= sa[h] * s.x; v[4 * j + 2 * h + 1] *= sa[h] * s.y; }
+        });
+    if (p.ln_stats)
+        col_pass<NJ>(p.ln_colsum, n0, p.N, full, [&](int j, float2 s) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                v[4 * j + 2 * h] = fmaf(v[4 * j + 2 * h], st[h].x, -st[h].y * s.x);
+                v[4 * j + 2 * h + 1] = fmaf(v[4 * j + 2 * h + 1], st[h].x, -st[h].y * s.y);
+            }
+        });
+    if (p.bias)
+        col_pass<NJ>(p.bias, n0, p.N, full, [&](int j, float2 s) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) { v[4 * j + 2 * h] += s.x; v[4 * j + 2 * h + 1] += s.y; }
+        });
+    if (p.rowvec) {
+        // one pass when both rows are in one batch (always in conv mode: a tile is one image's patch), else one per row
+        const bool one = rv[0] == rv[1];
+        col_pass<NJ>(rv[0], n0, p.N, full, [&](int j, float2 s) {
+            v[4 * j] += s.x; v[4 * j + 1] += s.y;
+            if (one) { v[4 * j + 2] += s.x; v[4 * j + 3] += s.y; }
+        });
+        if (!one)
+            col_pass<NJ>(rv[1], n0, p.N, full, [&](int j, float2 s) { v[4 * j + 2] += s.x; v[4 * j + 3] += s.y; });
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        if (!row[h].ok) continue;
+        const int r = r_lo + 8 * h;
+        const long long grow = row[h].grow;
         if (p.act == 2) {
             // GEGLU: accumulator columns come in groups of 32 = [16 value | 16 gate]; this thread holds value column
             // 8 b + cq (+1) of group g in block 4 g + b and its gate 16 columns later in block 4 g + b + 2
@@ -201,21 +273,8 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
                 if (nt * BN + g * 32 >= p.N) break;
 #pragma unroll
                 for (int b = 0; b < 2; ++b) {
-                    const int nv = nt * BN + g * 32 + b * 8 + cq;
-                    float xv0 = acc[4 * (4 * g + b) + 2 * h], xv1 = acc[4 * (4 * g + b) + 2 * h + 1];
-                    float gv0 = acc[4 * (4 * g + b + 2) + 2 * h], gv1 = acc[4 * (4 * g + b + 2) + 2 * h + 1];
-                    if constexpr (E::kFp8) {
-                        xv0 *= sa * __ldg(p.w_scale + nv); xv1 *= sa * __ldg(p.w_scale + nv + 1);
-                        gv0 *= sa * __ldg(p.w_scale + nv + 16); gv1 *= sa * __ldg(p.w_scale + nv + 17);
-                    }
-                    if (p.bias) {
-                        xv0 += __ldg(p.bias + nv); xv1 += __ldg(p.bias + nv + 1);
-                        gv0 += __ldg(p.bias + nv + 16); gv1 += __ldg(p.bias + nv + 17);
-                    }
-                    if (rv) {
-                        xv0 += __ldg(rv + nv); xv1 += __ldg(rv + nv + 1);
-                        gv0 += __ldg(rv + nv + 16); gv1 += __ldg(rv + nv + 17);
-                    }
+                    const float xv0 = v[4 * (4 * g + b) + 2 * h], xv1 = v[4 * (4 * g + b) + 2 * h + 1];
+                    const float gv0 = v[4 * (4 * g + b + 2) + 2 * h], gv1 = v[4 * (4 * g + b + 2) + 2 * h + 1];
                     float o0 = E::round(E::round(xv0) * E::round(gelu_erf_f(E::round(gv0))));
                     float o1 = E::round(E::round(xv1) * E::round(gelu_erf_f(E::round(gv1))));
                     const int c = g * 16 + b * 8 + cq;                 // output column within the tile's BN / 2
@@ -229,44 +288,12 @@ __device__ __forceinline__ void epilogue_m64(const GemmKernelParams& p, const fl
                 }
             }
         } else {
-            constexpr int NJ = BN / 8;
-            float v[NJ][2];
-#pragma unroll
-            for (int j = 0; j < NJ; ++j) { v[j][0] = acc[4 * j + 2 * h]; v[j][1] = acc[4 * j + 2 * h + 1]; }
-            // One branch-free pass per column operand: every load of a pass is issued before the first use, instead of one
-            // load-use round trip per column pair. Columns past N read column N - 1 (their results are never stored).
-            const auto col = [&](int j, int e) { const int n = nt * BN + 8 * j + cq + e; return n < p.N ? n : p.N - 1; };
-            if (E::kFp8 && p.w_scale) {     // (a run-time branch, like the passes below: it keeps the passes' loads apart)
-#pragma unroll
-                for (int j = 0; j < NJ; ++j)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) v[j][e] *= sa * __ldg(p.w_scale + col(j, e));
-            }
-            if (p.ln_stats) {
-                const float2 st = __ldg(p.ln_stats + grow);
-#pragma unroll
-                for (int j = 0; j < NJ; ++j)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) v[j][e] = fmaf(v[j][e], st.x, -st.y * __ldg(p.ln_colsum + col(j, e)));
-            }
-            if (p.bias) {
-#pragma unroll
-                for (int j = 0; j < NJ; ++j)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) v[j][e] += __ldg(p.bias + col(j, e));
-            }
-            if (rv) {
-#pragma unroll
-                for (int j = 0; j < NJ; ++j)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) v[j][e] += __ldg(rv + col(j, e));
-            }
 #pragma unroll
             for (int j = 0; j < NJ; ++j) {
                 const int n = nt * BN + 8 * j + cq;
                 if (n >= p.N) break;
                 const bool n1ok = n + 1 < p.N;
-                float v0 = v[j][0], v1 = v[j][1];
+                float v0 = v[4 * j + 2 * h], v1 = v[4 * j + 2 * h + 1];
                 if (p.act == 1) { v0 = silu_f(E::round(v0)); v1 = silu_f(E::round(v1)); }
                 if (p.residual) {
                     const float2 rr = E::unpack2(STAGED ? ld_shared_u32(frag + stage_off(r, 8 * j + cq)) : load_res_bits<E>(p, grow, n, n1ok));

@@ -98,6 +98,7 @@ KSWEEP = (
     ("res 33792x1280", "gemm", 33792, 1280, "bias+res", (640, 1280, 1920, 2560), 1280),
     ("res 135168x640", "gemm", 135168, 640, "bias+res", (320, 640, 960, 1280), 640),
     ("ln 33792x3840", "gemm", 33792, 3840, "ln+bias", (640, 1280, 1920, 2560), 1280),
+    ("ln 135168x1920", "gemm", 135168, 1920, "ln+bias", (320, 640, 960, 1280), 640),
     ("conv 33x64x64->640", "conv", (33, 64, 64), 640, "bias+rowvec", (2304, 3456, 4608, 5760), 5760),
 )
 
